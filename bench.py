@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — views/sec of the MUSt3R multi-view inference hot path on B200 (BASELINE.json metric).
+"""bench.py — views/sec of the MUSt3R multi-view inference hot path on H100 (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--config c3|c2|c4|c5] [--dtype bf16|fp16] [--impl reference]
+                    [--dump-outputs DIR]
 
 A "step" is one whole job of a configuration of BASELINE.json (SURVEY.md §8d), on synthetic views and random-init
 ViT-L encoder / ViT-B memory decoder:
@@ -16,10 +17,12 @@ ViT-L encoder / ViT-B memory decoder:
 
 Prints ONE JSON line (rank 0).  `value` = device-timed views/s with inputs resident in HBM; `e2e` = the same job through
 the public engine API from pinned HOST images to HOST results (H2D / D2H inside the timed region); `parity` = rel-L2 of
-the timed job's own outputs against the UNMODIFIED reference (baseline/_ref) run in fp32 on the same GPU, for fp16 and
+the timed job's own outputs against the UNMODIFIED reference (oracle/_ref) run in fp32 on the same GPU, for fp16 and
 bf16 operands; `roofline` = per-kernel-category achieved TFLOP/s vs the measured bf16 peak; `cpu_baseline` = the
 unmodified reference's engine on this box's host cores on a bounded sample; `records` = the other configurations.
-`--impl reference` times that CPU path alone.
+`--impl reference` times that CPU path alone.  `--dump-outputs DIR` writes what the timed job returned in its last timed
+step (pts3d, pts3d_local, conf of every view, float32; a fixed seeded sample where an array exceeds its share of 64 MB) as
+DIR/<name>.npy, so that two builds can be compared output for output on identical inputs.
 """
 import argparse
 import json
@@ -30,6 +33,7 @@ import sys
 import threading
 import time
 
+import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
@@ -160,7 +164,7 @@ def reference_available():
 
 
 def build_reference(size, device, curope_shim):
-    """The UNMODIFIED reference's classes (baseline/_ref, installed by tools/install_reference.py) with the synthetic weights."""
+    """The UNMODIFIED reference's classes (oracle/_ref, installed by oracle/install_reference.py) with the synthetic weights."""
     from baseline import ref_loader
     from must3r_b200 import synthetic as syn
     ref = ref_loader.load_reference(curope_shim=curope_shim)
@@ -174,7 +178,7 @@ def build_reference(size, device, curope_shim):
 def cpu_reference_job(cfg, n_views, threads):
     """The reference's own engine on host cores (must3r/engine/inference.py:370 inference_multi_ar, SDPA branch, PyTorch RoPE
     fallback, fp32): the first `n_views` views of the configuration = encoder + 2-view init + (n-2) one-view updates +
-    render of the n views + activation.  Falls back to the oracle port (kind "port") when baseline/_ref is absent."""
+    render of the n views + activation.  Falls back to the oracle port (kind "port") when oracle/_ref is absent."""
     from must3r_b200 import synthetic as syn
     torch.set_num_threads(threads)
     H, W, size = cfg["H"], cfg["W"], cfg["size"]
@@ -217,7 +221,7 @@ def run_reference_arm(args, rank, world):
         job()
     dt = (time.perf_counter() - t0) / args.steps
     v = n / dt
-    what = "unmodified reference (baseline/_ref, must3r.engine.inference_multi_ar, fp32, SDPA, RoPE fallback)" if kind == "reference" else "oracle port (baseline/_ref missing)"
+    what = "unmodified reference (oracle/_ref, must3r.engine.inference_multi_ar, fp32, SDPA, RoPE fallback)" if kind == "reference" else "oracle port (oracle/_ref missing)"
     sample = f"{n} of the {cfg['V']} views per step ({cfg['H']}x{cfg['W']}: encoder + 2-view init + {n - 2} one-view update(s) + render {n} + activation), {what}"
     print(json.dumps({
         "impl": "reference", "metric": "views/sec at 512x384 (ViT-L enc / ViT-B dec)", "value": v, "unit": "views/s",
@@ -228,6 +232,24 @@ def run_reference_arm(args, rank, world):
         "cpu_baseline": {"value": v, "unit": "views/s", "cores": threads, "kind": kind, "sample": sample},
         "e2e": {"value": v, "unit": "views/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
         "gpu_launches": 0}))
+
+
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, pm):
+    """The arrays a caller of the timed job receives (per-view dicts of pts3d / pts3d_local / conf), stacked over the views
+    as float32 .npy files.  An array larger than its share of DUMP_BYTES is replaced by a fixed sample: the same seeded
+    element positions (sorted) every run, so two builds are compared element for element."""
+    os.makedirs(out_dir, exist_ok=True)
+    names = sorted(pm[0].keys())
+    cap = DUMP_BYTES // 4 // len(names)                      # float32 elements per array
+    for name in names:
+        a = torch.stack([d[name] for d in pm]).float().cpu().flatten()
+        if a.numel() > cap:
+            idx = torch.randperm(a.numel(), generator=torch.Generator().manual_seed(0))[:cap].sort().values
+            a = a[idx]
+        np.save(os.path.join(out_dir, f"{name}.npy"), a.numpy().astype(np.float32))
 
 
 # ------------------------------------------------------------------------------------------------ GPU arm
@@ -244,6 +266,8 @@ def main():
     ap.add_argument("--no-records", action="store_true", help="skip the extra configurations (records)")
     ap.add_argument("--no-parity", action="store_true")
     ap.add_argument("--stream-frames", type=int, default=1000)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32, at most 64 MB in all)")
     ap.add_argument("--encoder-mode", default="precomputed", choices=["engine", "precomputed"],
                     help="precomputed (default): engine.encoder_multi_ar over all views first, then the decoder chain (features handed to "
                          "the engine); engine: encoder_precomputed_features=None, the engine encodes the missing views itself (up front, batched)")
@@ -390,7 +414,7 @@ def main():
         """rel-L2 of the job's rendered outputs (raw head, pts3d, conf) vs the unmodified reference run in fp32 on this GPU
         (TF32 off, its RoPE served by must3r_b200.compat.curope), for fp16 and bf16 operands.  Single-GPU chain configs."""
         if args.no_parity or not reference_available():
-            return {"unavailable": "baseline/_ref missing" if not args.no_parity else "--no-parity"}
+            return {"unavailable": "oracle/_ref missing" if not args.no_parity else "--no-parity"}
         V, H, W = cfg["V"], cfg["H"], cfg["W"]
         torch.backends.cuda.matmul.allow_tf32 = False
         torch.backends.cudnn.allow_tf32 = False
@@ -409,7 +433,7 @@ def main():
             r_post = ref.engine.postprocess(r_raw, ref.model.ActivationType.NORM_EXP)
         del renc, rdec
         rel = lambda a, b: float((a.double() - b.double()).norm() / b.double().norm())  # noqa: E731
-        out = {"against": "unmodified reference (baseline/_ref) fp32 on this GPU, TF32 off, same schedule through its own engine",
+        out = {"against": "unmodified reference (oracle/_ref) fp32 on this GPU, TF32 off, same schedule through its own engine",
                "views": V, "reference_gpu_ms_per_job": round(t_ref * 1e3, 1)}
         for dt in (torch.float16, torch.bfloat16):
             set_precision(dt)
@@ -428,7 +452,7 @@ def main():
         (fp32, rank 0's GPU): rounds of one-view updates against the memory of the previous rounds, tokens appended in rank
         order, then render (tests/test_sharded_cpu.py composes the oracle the same way)."""
         if args.no_parity or not reference_available():
-            return {"unavailable": "baseline/_ref missing" if not args.no_parity else "--no-parity"}
+            return {"unavailable": "oracle/_ref missing" if not args.no_parity else "--no-parity"}
         counts = meta["counts"]
         raw = lambda pm: {"raw": pm}  # noqa: E731
         res = {}
@@ -484,8 +508,14 @@ def main():
         job()
     barrier()
     launches0 = lib.m3r_launch_count()
-    ms = timed(job, args.steps, 0, sampler=clk)
+    last = {}
+
+    def headline_job():
+        last["out"] = job()
+    ms = timed(headline_job, args.steps, 0, sampler=clk)
     launches = (lib.m3r_launch_count() - launches0) // args.steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["out"])
     value = meta["views"] / (ms / 1e3)
 
     # ---- end to end: pinned host images -> host results (H2D / D2H inside the timed region)
@@ -523,13 +553,13 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:  # noqa: BLE001
             pass
-        peak = float(peaks.get("bf16_tflops_sustained", 1590.0)) if peaks else 1590.0
-        peak_src = "measured (MEASURED_PEAKS.json bf16_tflops_sustained: kernels timed inside a long step)" if peaks else "fallback 1.59 PFLOP/s"
+        peak = float(peaks.get("bf16_tflops_sustained", 989.0)) if peaks else 989.0
+        peak_src = "measured (MEASURED_PEAKS.json bf16_tflops_sustained: kernels timed inside a long step)" if peaks else "H100 SXM data sheet, dense BF16 989 TFLOP/s at 700 W (not measured)"
         tensor_cats = [c for c in cats if prof[c]["flops"] > 0]
         dom = max(tensor_cats, key=lambda c: prof[c]["ms"])
         ach = prof[dom]["flops"] / (prof[dom]["ms"] * 1e-3) / 1e12 if prof[dom]["ms"] > 0 else 0.0
-        # dram__bytes_read + dram__bytes_write of ONE representative launch of the dominant category, taken from the committed
-        # `ncu --set full` captures (bench.py cannot run ncu itself); the file names the launch shape and the summary it came from
+        # dram__bytes_read + dram__bytes_write of ONE representative launch of the dominant category, from an optional
+        # profiles/r02_ncu_traffic.json (bench.py cannot run a profiler itself); the file names the launch shape and its source
         try:
             traffic = json.load(open(os.path.join(ROOT, "profiles", "r02_ncu_traffic.json"))).get(dom, {})
         except Exception:  # noqa: BLE001
@@ -637,7 +667,7 @@ def main():
             "higher_is_better": True, "scaling": "strong" if args.config == "c4" else "weak", "vs_baseline": None, "dtype": args.dtype, "data": "synthetic",
             "config": {"workload": cfg["label"] + (", random-init ViT-L enc / ViT-B dec" if True else ""), "config_id": args.config,
                        "global_views": meta["views"], "parallelism": par, "encoder_mode": args.encoder_mode,
-                       "l2": "working set (1.7 GB of 16-bit weights + activations + memory tokens) exceeds the 126 MB L2; no explicit flush"},
+                       "l2": "working set (1.7 GB of 16-bit weights + activations + memory tokens) exceeds the 50 MB L2; no explicit flush"},
             "e2e": {"value": meta["views"] / (ms_e2e / 1e3), "unit": "views/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                     "ms_per_step": ms_e2e},
             "gpu_launches": int(launches), "kernel_time_shares": shares, "roofline": roof, "parity": parity, "records": records,

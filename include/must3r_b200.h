@@ -1,5 +1,5 @@
 /*
- * must3r_b200 — C ABI of the B200-native MUSt3R inference hot path (libm3r_b200.so).
+ * must3r_b200 — C ABI of the H100-native MUSt3R inference hot path (libm3r_b200.so).
  *
  * Plain pointers and sizes only (no torch types).  All pointers are DEVICE pointers unless noted;
  * buffers are borrowed for the duration of the call; work is enqueued on `stream` (the caller's current
@@ -51,7 +51,7 @@ int m3r_prof_read(double* out);
 int m3r_debug_trace(void* buf);
 
 /* ---------------------------------------------------------------------------------------------------
- * Linear layer y = act(x W^T + b) (+ residual) on tcgen05 tensor cores.
+ * Linear layer y = act(x W^T + b) (+ residual) on wgmma tensor cores.
  * Replaces nn.Linear / croco Mlp call sites: must3r/model/blocks/attention.py:88-89,108-111,
  * dust3r/croco/models/blocks.py:67-70, must3r/model/decoder.py:50, must3r/model/blocks/head.py:67,
  * and, with rope_tab != NULL, the fused qkv projection + curope.rope_2d
@@ -163,7 +163,7 @@ int m3r_rope_2d(void* tokens, int32_t dtype /*0 f32,1 f16,2 bf16*/, int32_t B, i
                 int64_t sB, int64_t sN, int64_t sH, const int64_t* pos, float base, float fwd, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
- * FlashAttention-style softmax(Q K^T / 8) V, head_dim 64, on tcgen05 (S and P·V in TMEM, online softmax).
+ * FlashAttention-style softmax(Q K^T / 8) V, head_dim 64, on wgmma (S, P and O in registers, online softmax).
  * Replaces CoreAttention.attention (must3r/model/blocks/attention.py:37-79) for both self-attention and
  * the memory cross-attention, including the "drop each image's own new tokens" mask of
  * MUSt3R.make_mem_mask (must3r/model/decoder.py:119-139) and the torch.cat / expand / boolean gather of

@@ -1,4 +1,4 @@
-"""must3r_b200: B200-native (sm_100a) implementation of the MUSt3R multi-view inference hot path.
+"""must3r_b200: H100-native (sm_90a) implementation of the MUSt3R multi-view inference hot path.
 
 Public surface mirrors the reference: ``must3r_b200.model`` (load_model, Dust3rEncoder, MUSt3R, ...) and
 ``must3r_b200.engine`` (inference_multi_ar, inference_video_multi_ar, inference, postprocess, ...).

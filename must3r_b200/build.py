@@ -1,7 +1,7 @@
-"""Build libm3r_b200.so (hand-written sm_100a kernels + C ABI) in-tree with nvcc.
+"""Build libm3r_b200.so (hand-written sm_90a kernels + C ABI) in-tree with nvcc.
 
-nvcc cross-compiles for sm_100a without a GPU; the resulting .so is git-ignored but travels to the GPU box
-with the gpurun snapshot.  Usage: ``python -m must3r_b200.build [--force]``.
+nvcc cross-compiles for sm_90a (H100) without a GPU; the resulting .so and objects are git-ignored build products.
+Usage: ``python -m must3r_b200.build [--force]``.
 """
 from __future__ import annotations
 
@@ -14,7 +14,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libm3r_b200.so")
 SOURCES = ["runtime.cu", "elementwise.cu", "gemm.cu", "attention.cu", "model.cu"]  # missing files are skipped
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = GENCODE + ["-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC"]
 
 
@@ -63,7 +64,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         res = list(ex.map(compile_one, srcs))
     objs = [o for o, _ in res]
     if force or any(c for _, c in res) or _stale(OUT, objs):
-        cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", OUT] + objs
+        cmd = [nvcc, "-shared"] + GENCODE + ["-o", OUT] + objs
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

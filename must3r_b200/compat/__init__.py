@@ -4,5 +4,5 @@
                                   (dust3r/croco/models/curope/curope.cpp:49-69, curope2d.py:32-39).
 ``must3r_b200.compat.attention``  ``toggle_memory_efficient_attention`` / ``has_xformers`` of
                                   must3r/model/blocks/attention.py:5-27 and an ``attention()`` with the signature of
-                                  ``CoreAttention.attention`` (:37) running on the tcgen05 kernel.
+                                  ``CoreAttention.attention`` (:37) running on the wgmma kernel.
 """

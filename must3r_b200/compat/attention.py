@@ -1,8 +1,8 @@
-"""Attention seam of the reference (must3r/model/blocks/attention.py:5-79) on the tcgen05 kernel.
+"""Attention seam of the reference (must3r/model/blocks/attention.py:5-79) on the wgmma kernel.
 
 ``toggle_memory_efficient_attention`` / ``is_memory_efficient_attention_enabled`` / ``has_xformers`` keep the names
 callers flip at start-up (must3r/demo/gradio.py, must3r/slam/slam.py, eval.py call ``toggle_memory_efficient_attention``):
-here they only record the flag - there is one attention backend, the sm_100a kernel, and no xFormers dependency.
+here they only record the flag - there is one attention backend, the sm_90a kernel, and no xFormers dependency.
 ``attention(q, k, v)`` has the calling convention of ``CoreAttention.attention`` after RoPE (:37,:66-79): ``[B,H,N,64]``
 16-bit CUDA tensors in, ``[B,Nq,H*64]`` out; it is what the one-line patch of INTEGRATION.md §4 calls.
 """

@@ -1,24 +1,17 @@
-// FlashAttention-style softmax(Q K^T * scale) V for head_dim 64 on sm_100a tensor cores (tcgen05 + TMEM).
+// FlashAttention-style softmax(Q K^T * scale) V for head_dim 64 on sm_90a tensor cores (wgmma).
 //
 // One CTA = one (batch, head, QT x 128 queries [, key split]).  QT = 2 for throughput shapes: the two query tiles
-// share every K / V tile that TMA brings in (half the L2->smem traffic) and ping-pong on the tensor pipe, so one
-// tile's softmax overlaps the other's MMAs.  Roles:
-//   warps 0..4*QT-1 : (4*CS*QT warps with the optional column-split variant, see AttnCfg) softmax warpgroup per
-//                     query tile -- ONE query row per thread (TMEM lane == row, so row max /
-//                     row sum need no shuffles); single pass over a 128-key S row held in registers: row max, exp2
-//                     with the scale folded in, row sum, pack P to 16-bit into its own TMEM columns.  As soon as
-//                     the row is in registers the S columns are handed back, so Q K^T of tile j+1 runs under the
-//                     exponentials of tile j.
-//   warp 4*QT       : TMA producer -- Q tiles once, then K and V tiles (128 keys x 64) through mbarrier rings.
+// share every K / V tile that TMA brings in (half the L2->smem traffic).  Roles:
+//   warps 0..8*QT-1 : 2*QT consumer warpgroups, 64 query rows each.  Per 128-key tile, in CS column slices (2 x 64 keys by default):
+//                     S[64 x 64] = Q K^T (wgmma, both operands K-major smem, fp32 scores in registers), row max over
+//                     the quad of threads sharing a row, exp2 with the scale folded in, row sums, P packed to 16-bit
+//                     straight into the register A operand of O += P V (wgmma with V as an MN-major smem B operand:
+//                     V is consumed in its natural [keys, d] layout -- no transpose anywhere in the pipeline).
+//                     The warpgroups run independently, so one's softmax overlaps another's MMAs.
+//   warp 8*QT       : TMA producer -- Q tiles once, then K and V tiles (128 keys x 64) through mbarrier rings.
 //                     3-D tensor maps: rows beyond Nk read as zeros even inside over-allocated memory buffers.
-//   warps 4*QT+1..  : one single-thread MMA issuer per query tile (the first also allocates TMEM):
-//                     S = Q K^T (both operands K-major smem),
-//                     O += P V with P as the TMEM A operand and V as an MN-major smem B operand (V is consumed in
-//                     its natural [keys, d] layout -- no transpose anywhere in the pipeline).
-// O accumulates in TMEM across key tiles.  The running max used in the exponent is only refreshed when the true
-// row max grew by more than 2^8 (lazy rescaling): the rare refresh multiplies O in TMEM by the correction factor;
-// the final O / l is mathematically unchanged.
-// TMEM columns per query tile x (256 each): S [0,128)  P [128,192) (packed 16-bit pairs)  O [192,256).
+// O accumulates in registers across key tiles.  The running max used in the exponent is only refreshed when the true
+// row max grew by more than 2^8 (lazy rescaling); the final O / l is mathematically unchanged.
 //
 // Keys come from two segments (stored memory + this step's new tokens) so the reference's torch.cat of the memory
 // (decoder.py:306) never happens; a per-batch skip range implements make_mem_mask (decoder.py:119-139): fully
@@ -39,17 +32,15 @@ constexpr int HD = 64;
 constexpr int TILE_BYTES = 128 * HD * 2;     // 16 KB
 constexpr float RESCALE_THRESHOLD = 8.0f;    // log2 units
 
-// CS = softmax warpgroups per query tile ("column split"): with CS = 2 two warpgroups own the same 128 rows (TMEM lanes)
-// and half of the 128 score columns each, so the per-tile chain  S load -> max -> exp -> P store  of a thread is half
-// as long and twice as many warps hide each other's MUFU / TMEM latencies; the row maximum is exchanged through smem.
-template <int QT, int CS> struct AttnCfg {
+template <int QT> struct AttnCfg {
   static constexpr int KS = QT == 2 ? 3 : 2;                       // K / V ring depth
-  static constexpr int SM_WARPS = 4 * CS * QT;                     // softmax warps
-  static constexpr int THREADS = 32 * (SM_WARPS + 1 + QT);         // + TMA warp + one MMA issuer per tile
-  static constexpr int XCHG_BYTES = CS == 2 ? QT * 2 * 2 * AT_BM * 4 : 0;   // [tile][parity][half][row] fp32
-  static constexpr int SMEM = (QT + 2 * KS) * TILE_BYTES + 1024 + 256 + XCHG_BYTES;
-  static constexpr int TMEM_COLS = QT == 2 ? 512 : 256;
+  static constexpr int THREADS = 32 * (8 * QT + 1);                // consumer warpgroups + TMA warp
+  static constexpr int SMEM = (QT + 2 * KS) * TILE_BYTES + 1024 + 256;
 };
+constexpr int OSTR = HD + 1;                 // fp32 row stride of the O tile staged for the epilogue (conflict-free reads)
+// the staged O tiles + (m, l) rows overlay the Q and K stages
+static_assert(AT_BM * OSTR * 4 + AT_BM * 8 <= (1 + AttnCfg<1>::KS) * TILE_BYTES, "O staging must fit over the Q / K stages");
+static_assert(2 * (AT_BM * OSTR * 4 + AT_BM * 8) <= (2 + AttnCfg<2>::KS) * TILE_BYTES, "O staging must fit over the Q / K stages");
 
 struct AttnParams {
   int Nq, Nk0, Nk1;
@@ -124,44 +115,6 @@ __device__ __forceinline__ float ex2(float x) {
   return y;
 }
 
-// ---- packed fp32x2 arithmetic (FFMA2 / FADD2): two lanes per issue slot on the FMA pipe
-__device__ __forceinline__ uint64_t pk2(float a, float b) { uint64_t r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
-__device__ __forceinline__ void up2(uint64_t v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ uint64_t fma2(uint64_t a, uint64_t b, uint64_t c) { uint64_t d; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c)); return d; }
-__device__ __forceinline__ uint64_t add2(uint64_t a, uint64_t b) { uint64_t d; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-__device__ __forceinline__ uint64_t sub2(uint64_t a, uint64_t b) { uint64_t d; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-
-// 2^x for a pair on the FMA/ALU pipes instead of the MUFU: Cody-Waite split x = n + f (round to nearest via the
-// 1.5*2^23 magic add), degree-3 minimax polynomial for 2^f on [-0.5,0.5] (max rel. error 1.0e-4, below the 16-bit
-// rounding of P), n added straight into the exponent field.  At head_dim 64 the 16/clk/SM MUFU is the binding unit
-// of attention (DESIGN.md §6): POLY of every 8 exponential pairs take this path (shipped default 1, M3R_ATTN_POLY=0..3;
-// more than 1 of 8 is slower - the softmax warps run out of issue slots, profiles/r01_attention_variants.txt).
-struct PolyC { uint64_t magic, c3, c2, c1, c0; };
-__device__ __forceinline__ PolyC make_polyc() {
-  PolyC c;
-  c.magic = pk2(12582912.f, 12582912.f);
-  c.c3 = pk2(0.0559220351f, 0.0559220351f);
-  c.c2 = pk2(0.242640078f, 0.242640078f);
-  c.c1 = pk2(0.693121016f, 0.693121016f);
-  c.c0 = pk2(0.999924481f, 0.999924481f);
-  return c;
-}
-__device__ __forceinline__ void ex2_poly2(uint64_t v, const PolyC& c, float& r0, float& r1) {
-  float x0, x1;
-  up2(v, x0, x1);
-  v = pk2(fmaxf(x0, -125.f), fmaxf(x1, -125.f));          // -inf (masked) -> 2^-125, which rounds to 0 in 16 bits
-  const uint64_t t = add2(v, c.magic);
-  const uint64_t f = sub2(v, sub2(t, c.magic));
-  uint64_t q = fma2(f, c.c3, c.c2);
-  q = fma2(q, f, c.c1);
-  q = fma2(q, f, c.c0);
-  float q0, q1, t0, t1;
-  up2(q, q0, q1);
-  up2(t, t0, t1);
-  r0 = __uint_as_float(__float_as_uint(q0) + (__float_as_uint(t0) << 23));
-  r1 = __uint_as_float(__float_as_uint(q1) + (__float_as_uint(t1) << 23));
-}
-
 template <bool BF16> __device__ __forceinline__ uint32_t packp(float lo, float hi) {
   uint32_t r;
   if (BF16) asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
@@ -169,16 +122,17 @@ template <bool BF16> __device__ __forceinline__ uint32_t packp(float lo, float h
   return r;
 }
 
-template <bool BF16, int QT, int POLY, int CS>
-__global__ void __launch_bounds__(AttnCfg<QT, CS>::THREADS, QT == 1 ? 2 : 1)
+template <bool BF16, int QT, int CS>
+__global__ void __launch_bounds__(AttnCfg<QT>::THREADS, QT == 1 ? 2 : 1)
 attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK0,
             const __grid_constant__ CUtensorMap tmV0, const __grid_constant__ CUtensorMap tmK1,
             const __grid_constant__ CUtensorMap tmV1, const AttnParams p) {
-  using Cfg = AttnCfg<QT, CS>;
+  using Cfg = AttnCfg<QT>;
   constexpr int KS = Cfg::KS;
-  constexpr int TMA_WARP = Cfg::SM_WARPS, MMA_WARP = Cfg::SM_WARPS + 1;      // issuers: warps MMA_WARP .. MMA_WARP+QT-1
-  constexpr int NC = AT_BN / CS;                                // score columns per softmax thread
-  constexpr int SMT = 128 * CS;                                 // softmax threads per query tile
+  constexpr int NWG = 2 * QT;                                   // consumer warpgroups (64 query rows each)
+  constexpr int CT = 128 * NWG;                                 // consumer threads
+  constexpr int TMA_WARP = 4 * NWG;
+  constexpr int SW = AT_BN / CS;                                // score columns per softmax pass
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;                                   // QT tiles
@@ -190,12 +144,6 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
   uint64_t* k_empty = k_full + KS;     // [KS]
   uint64_t* v_full = k_empty + KS;     // [KS]
   uint64_t* v_empty = v_full + KS;     // [KS]
-  uint64_t* s_full = v_empty + KS;     // [2] MMA -> softmax x : S_x(j) ready
-  uint64_t* s_free = s_full + 2;       // [2] softmax x -> MMA : S_x(j) is in registers, the columns may be overwritten
-  uint64_t* p_full = s_free + 2;       // [2] softmax x -> MMA : P_x(j) stored (and O_x rescaled if needed)
-  uint64_t* o_done = p_full + 2;       // [2] MMA -> softmax x : P_x(j) V(j) accumulated into O_x, P columns free again
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_done + 2);
-  float* xchg = reinterpret_cast<float*>(smem + (QT + 2 * KS) * TILE_BYTES + 256);   // CS == 2 only
 
   M3R_TR(const unsigned long long t_entry = p.trace ? gtime_ns() : 0ull;)
   const int warp = threadIdx.x >> 5;
@@ -204,9 +152,7 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
   const int kvb = b / p.kv_group;
   const int lo = p.skip_len > 0 ? p.skip_lo + (b % p.kv_group) * p.skip_step : 0;
   const int hi = p.skip_len > 0 ? lo + p.skip_len : 0;
-  // number of query tiles of this CTA that hold at least one real query
   const int q0 = qblk * QT * AT_BM;
-  const int nqt = (QT == 2 && q0 + AT_BM < p.Nq) ? 2 : 1;
 
   // this CTA's share [i0, i1) of the enumerated key tiles
   const TileMap tiles(p.Nk0, p.Nk1, lo, hi);
@@ -220,23 +166,18 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
     tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK0); tma_prefetch_desc(&tmV0);
     if (p.Nk1 > 0) { tma_prefetch_desc(&tmK1); tma_prefetch_desc(&tmV1); }
     mbar_init(q_full, 1);
-    for (int s = 0; s < KS; ++s) { mbar_init(&k_full[s], 1); mbar_init(&k_empty[s], nqt); mbar_init(&v_full[s], 1); mbar_init(&v_empty[s], nqt); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&s_full[s], 1); mbar_init(&s_free[s], SMT); mbar_init(&p_full[s], SMT); mbar_init(&o_done[s], 1); }
+    for (int s = 0; s < KS; ++s) { mbar_init(&k_full[s], 1); mbar_init(&k_empty[s], NWG); mbar_init(&v_full[s], 1); mbar_init(&v_empty[s], NWG); }
     fence_mbar_init();
   }
-  if (warp == MMA_WARP) { tmem_alloc(tmem_slot, Cfg::TMEM_COLS); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   griddep_wait();
   griddep_launch();
 
   if (warp == TMA_WARP) {
     // ------------------------------------------------------------------ TMA producer
     if (elect_one() && n_tiles > 0) {
-      mbar_arrive_expect_tx(q_full, nqt * TILE_BYTES);
-      for (int x = 0; x < nqt; ++x) tma_load_3d(sQ + x * TILE_BYTES, &tmQ, q_full, h * HD, q0 + x * AT_BM, b);
+      mbar_arrive_expect_tx(q_full, QT * TILE_BYTES);
+      for (int x = 0; x < QT; ++x) tma_load_3d(sQ + x * TILE_BYTES, &tmQ, q_full, h * HD, q0 + x * AT_BM, b);
       for (int j = 0; j < n_tiles; ++j) {
         const TileIt it = tiles.get(i0 + j);
         const int st = j % KS;
@@ -251,341 +192,260 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
         tma_load_3d(sV + st * TILE_BYTES, mv, &v_full[st], h * HD, it.t * AT_BN, kvb);
       }
     }
-  } else if (warp >= MMA_WARP && warp < MMA_WARP + nqt) {
-    // ------------------------------------------------------------------ MMA issuer of query tile x (one thread)
-    // One issuer per query tile: the two softmax warpgroups progress independently (neither waits for the other's
-    // P), they only share the K / V stages, released when every issuer has committed its last read.
-    constexpr uint32_t bf = BF16 ? 1u : 0u;
-    constexpr uint32_t idesc_qk = make_idesc(AT_BM, AT_BN, bf, 0, 0);   // S[128 x 128] = Q (K-major) * K^T (K-major)
-    constexpr uint32_t idesc_pv = make_idesc(AT_BM, HD, bf, 0, 1);      // O[128 x 64] += P (TMEM)   * V (MN-major)
-    const int x = warp - MMA_WARP;
-    if (n_tiles > 0 && (threadIdx.x & 31) == 0) {
-      const uint64_t qdesc = smem_desc_sw128(smem_u32(sQ + x * TILE_BYTES));
-      const uint64_t kdesc0 = smem_desc_sw128(smem_u32(sK));
-      const uint64_t vdesc0 = smem_desc_sw128(smem_u32(sV));
-      const uint32_t s_tmem = tmem_base + x * 256, p_tmem = s_tmem + 128, o_tmem = s_tmem + 192;
-      auto issue_qk = [&](int j) {                               // S_x = Q_x K(j)^T
-        const int st = j % KS;
-        const uint64_t kdesc = kdesc0 + (uint64_t)((st * TILE_BYTES) >> 4);
-#pragma unroll
-        for (int k = 0; k < HD / 16; ++k) umma_ss(s_tmem, qdesc + 2 * k, kdesc + 2 * k, idesc_qk, k ? 1u : 0u);
-        umma_commit(&s_full[x]);
-        umma_commit(&k_empty[st]);                               // this issuer's only read of the K tile
-      };
-      auto issue_pv = [&](int j) {                               // O_x (+)= P_x(j) V(j)
-        const int st = j % KS;
-        const uint64_t vdesc = vdesc0 + (uint64_t)((st * TILE_BYTES) >> 4);
-#pragma unroll
-        for (int k = 0; k < AT_BN / 16; ++k) {
-          // 16 keys per MMA: P advances 8 TMEM columns (packed pairs), V advances 16 rows = 2048 B
-          umma_ts(o_tmem, p_tmem + k * 8, vdesc + (uint64_t)(k * 128), idesc_pv, (j | k) ? 1u : 0u);
-        }
-        umma_commit(&o_done[x]);
-        umma_commit(&v_empty[st]);
-      };
-      M3R_TR(unsigned long long* trm = (p.trace && x == 0) ? p.trace + 128ull * ((blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) + 64 : nullptr;)
-      mbar_wait(q_full, 0);
-      mbar_wait(&k_full[0], 0);
-      tc_fence_after();
-      issue_qk(0);
-      for (int j = 0; j < n_tiles; ++j) {
-        if (j + 1 < n_tiles) {
-          mbar_wait(&k_full[(j + 1) % KS], ((j + 1) / KS) & 1);
-          M3R_TR(if (trm && j < 12) trm[4 * j] = gtime_ns();)
-          mbar_wait(&s_free[x], j & 1);                          // softmax holds S(j) in registers
-          M3R_TR(if (trm && j < 12) trm[4 * j + 1] = gtime_ns();)
-          tc_fence_after();
-          issue_qk(j + 1);                                       // runs under the exponentials of tile j
-        }
-        mbar_wait(&v_full[j % KS], (j / KS) & 1);
-        mbar_wait(&p_full[x], j & 1);
-        M3R_TR(if (trm && j < 12) trm[4 * j + 2] = gtime_ns();)
-        tc_fence_after();
-        issue_pv(j);
-        M3R_TR(if (trm && j < 12) trm[4 * j + 3] = gtime_ns();)
-      }
-    }
-  } else if (warp < 4 * CS * nqt) {
-    // ------------------------------------------------------------------ softmax warpgroup(s) of query tile x
-    const int x = warp / (4 * CS);
-    const int half = (warp % (4 * CS)) >> 2;     // which NC-column half of the score tile (always 0 when CS == 1)
-    const int quarter = warp & 3;                // TMEM lane quarter = warp id % 4
-    const int lane = threadIdx.x & 31;
-    const int row = quarter * 32 + lane;
-    const int q_idx = q0 + x * AT_BM + row;
-    const uint32_t lane_addr = tmem_base + (uint32_t(quarter * 32) << 16);
-    const uint32_t s_addr = lane_addr + x * 256 + half * NC;
-    const uint32_t p_addr = lane_addr + x * 256 + 128 + half * (NC / 2);
-    const uint32_t o_addr = lane_addr + x * 256 + 192 + half * (HD / CS);
-    float* xq = xchg + x * (2 * 2 * AT_BM);      // [parity][half][row]
-    float m_used = -INFINITY;      // max currently folded into the exponent (raw score units)
-    float l_run = 0.f;
-    const PolyC polyc = make_polyc();
+    return;
+  }
 
-    M3R_TR(unsigned long long* tr = nullptr;
-           if (p.trace && row == 0 && x == 0 && half == 0)
-             tr = p.trace + 128ull * ((blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x);
-           if (tr) { tr[0] = t_entry; tr[1] = gtime_ns(); tr[2] = smid(); tr[3] = (unsigned long long)n_tiles; })
-    int j = 0;
-    for (; j < n_tiles; ++j) {
+  // ------------------------------------------------------------------ consumer warpgroup: 64 query rows
+  const int wg = warp >> 2;
+  const int x = wg >> 1;                       // query tile
+  const int wl = warp & 3, lane = threadIdx.x & 31;
+  const int fr = (wg & 1) * 64 + wl * 16 + (lane >> 2);     // fragment rows fr and fr + 8 of the query tile
+  const int fc = 2 * (lane & 3);                            // fragment column offset inside every 8-column block
+  float o[32];                                 // O[64 x 64] fragment
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m_used[2] = {-INFINITY, -INFINITY};    // max currently folded into the exponent (raw score units), rows fr, fr + 8
+  float l_run[2] = {0.f, 0.f};                 // this thread's share of the row sums (reduced over the quad at the end)
+  M3R_TR(unsigned long long* tr = nullptr;
+         if (p.trace && threadIdx.x == 0)
+           tr = p.trace + 128ull * ((blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x);
+         if (tr) { tr[0] = t_entry; tr[1] = gtime_ns(); tr[2] = smid(); tr[3] = (unsigned long long)n_tiles; })
+  if (n_tiles > 0) {
+    const uint64_t qdesc = smem_desc_sw128(smem_u32(sQ + x * TILE_BYTES + (wg & 1) * 64 * 128));
+    mbar_wait(q_full, 0);
+    for (int j = 0; j < n_tiles; ++j) {
       const TileIt it = tiles.get(i0 + j);
-      mbar_wait(&s_full[x], j & 1);
+      const int st = j % KS;
+      const uint32_t ph = (j / KS) & 1;
+      mbar_wait(&k_full[st], ph);
       M3R_TR(if (tr && j < 12) tr[8 + 4 * j] = gtime_ns();)
-      tc_fence_after();
-      uint32_t raw[NC];
-#pragma unroll
-      for (int c = 0; c < NC / 32; ++c) tmem_ld32(s_addr + c * 32, *reinterpret_cast<uint32_t(*)[32]>(&raw[c * 32]));
-      tmem_wait_ld();
-      tc_fence_before();
-      mbar_arrive(&s_free[x]);                     // Q K^T of the next tile may overwrite S now
-      M3R_TR(if (tr && j < 12) tr[9 + 4 * j] = gtime_ns();)
-      if (it.mask) {
-#pragma unroll
-        for (int c = 0; c < NC; ++c) {
-          const int lc = half * NC + c;
-          const int g = it.g0 + lc;
-          const bool ok = lc < it.nvalid && !(g >= lo && g < hi);
-          if (!ok) raw[c] = 0xff800000u;            // -inf
-        }
-      }
-      float mx0 = -INFINITY, mx1 = -INFINITY, mx2 = -INFINITY, mx3 = -INFINITY;
-#pragma unroll
-      for (int c = 0; c < NC; c += 4) {
-        mx0 = fmaxf(mx0, __uint_as_float(raw[c]));
-        mx1 = fmaxf(mx1, __uint_as_float(raw[c + 1]));
-        mx2 = fmaxf(mx2, __uint_as_float(raw[c + 2]));
-        mx3 = fmaxf(mx3, __uint_as_float(raw[c + 3]));
-      }
-      float mx = fmaxf(fmaxf(mx0, mx1), fmaxf(mx2, mx3));
-      if (CS == 2) {
-        // the two threads of a row agree on the row maximum (hence on m_used and on every rescale decision); the buffer
-        // alternates with the tile parity, so a thread one tile ahead never overwrites a value its partner still reads
-        float* e = xq + (j & 1) * (2 * AT_BM);
-        e[half * AT_BM + row] = mx;
-        asm volatile("bar.sync %0, %1;" ::"r"(1 + x), "n"(SMT) : "memory");
-        mx = fmaxf(mx, e[(half ^ 1) * AT_BM + row]);
-      }
-      // lazy rescaling: refresh the folded max only when it is stale by more than 2^8
-      float alpha = 1.f;
-      bool refresh = false;
-      if (mx > -INFINITY && (m_used == -INFINITY || (mx - m_used) * p.sl2 > RESCALE_THRESHOLD)) {
-        refresh = true;
-        alpha = (m_used == -INFINITY) ? 0.f : ex2((m_used - mx) * p.sl2);
-        m_used = mx;
-      }
-      l_run *= alpha;
-      const float moff = (m_used == -INFINITY) ? 0.f : m_used * p.sl2;
-      const uint64_t sl2_2 = pk2(p.sl2, p.sl2), nmoff2 = pk2(-moff, -moff);
-      uint64_t rs0 = pk2(0.f, 0.f), rs1 = rs0;
-      // all exponentials of the tile first (the packed P values replace the scores in registers) ...
-      uint32_t pk[NC / 2];
-#pragma unroll
-      for (int c = 0; c < NC / 32; ++c) {
-#pragma unroll
-        for (int t = 0; t < 16; ++t) {
-          const uint64_t v = fma2(pk2(__uint_as_float(raw[c * 32 + 2 * t]), __uint_as_float(raw[c * 32 + 2 * t + 1])), sl2_2, nmoff2);
-          float a0, a1;
-          if (POLY > 0 && (t & 7) >= 8 - POLY) {   // POLY of every 8 pairs on the FMA / ALU pipes
-            ex2_poly2(v, polyc, a0, a1);
-          } else {
-            float x0, x1;
-            up2(v, x0, x1);
-            a0 = ex2(x0);
-            a1 = ex2(x1);
-          }
-          if (t & 1) rs1 = add2(rs1, pk2(a0, a1)); else rs0 = add2(rs0, pk2(a0, a1));
-          pk[c * 16 + t] = packp<BF16>(a0, a1);
-        }
-      }
-      // ... and only then the wait for P V (j-1): it must have consumed the P columns (and landed in O) before they are
-      // rewritten / O is rescaled, but its latency is now hidden behind the exponentials above instead of stalling the
-      // warpgroup between the row maximum and the first ex2.  Every phase of o_done is waited for, in order, so the
-      // parity wait is exact.
-      if (j > 0) {
-        mbar_wait(&o_done[x], (j - 1) & 1);
-        M3R_TR(if (tr && j < 12) tr[10 + 4 * j] = gtime_ns();)
-        tc_fence_after();
-        if (__any_sync(0xffffffffu, refresh)) {
+      const uint64_t kdesc = smem_desc_sw128(smem_u32(sK + st * TILE_BYTES));
+      const uint64_t vdesc = smem_desc_sw128(smem_u32(sV + st * TILE_BYTES));
+      // the 128-key tile in CS column slices of SW keys: S[64 x SW] = Q K_slice^T, online softmax, O += P V_slice
 #pragma unroll 1
-          for (int c = 0; c < 8 / CS; ++c) {          // rare path: small chunks keep the register footprint low
-            uint32_t o[8];
-            tmem_ld8(o_addr + c * 8, o);
-            tmem_wait_ld();
+      for (int hh = 0; hh < CS; ++hh) {
+        float s[SW / 2];
+        wgmma_fence();
 #pragma unroll
-            for (int d = 0; d < 8; ++d) o[d] = __float_as_uint(__uint_as_float(o[d]) * alpha);
-            tmem_st8(o_addr + c * 8, o);
+        for (int k = 0; k < HD / 16; ++k)        // K rows SW hh.. : +SW * 128 B; 16 head dims: +32 B
+          Wgmma<SW, BF16>::ss(s, qdesc + 2 * k, kdesc + (uint64_t)(hh * SW * 8) + 2 * k, k ? 1 : 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+        reg_fence(s);
+        if (hh == CS - 1 && wl == 0 && lane == 0) mbar_arrive(&k_empty[st]);      // this warpgroup's last read of the K tile
+        if (it.mask) {
+#pragma unroll
+          for (int i = 0; i < SW / 2; ++i) {
+            const int lc = hh * SW + (i >> 2) * 8 + fc + (i & 1);
+            const int g = it.g0 + lc;
+            if (!(lc < it.nvalid && !(g >= lo && g < hi))) s[i] = -INFINITY;
           }
         }
-      }
+        float alpha[2];
 #pragma unroll
-      for (int c = 0; c < NC / 32; ++c) tmem_st16(p_addr + c * 16, *reinterpret_cast<uint32_t(*)[16]>(&pk[c * 16]));
-      float r0, r1, r2, r3;
-      up2(rs0, r0, r1);
-      up2(rs1, r2, r3);
-      tmem_wait_st();
-      tc_fence_before();
-      mbar_arrive(&p_full[x]);
-      M3R_TR(if (tr && j < 12) tr[11 + 4 * j] = gtime_ns();)
-      l_run += (r0 + r1) + (r2 + r3);
+        for (int rr = 0; rr < 2; ++rr) {
+          float mx = -INFINITY;
+#pragma unroll
+          for (int i = 0; i < SW / 4; ++i) mx = fmaxf(mx, s[(i >> 1) * 4 + rr * 2 + (i & 1)]);
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+          // lazy rescaling: refresh the folded max only when it is stale by more than 2^8
+          alpha[rr] = 1.f;
+          if (mx > -INFINITY && (m_used[rr] == -INFINITY || (mx - m_used[rr]) * p.sl2 > RESCALE_THRESHOLD)) {
+            alpha[rr] = (m_used[rr] == -INFINITY) ? 0.f : ex2((m_used[rr] - mx) * p.sl2);
+            m_used[rr] = mx;
+          }
+          l_run[rr] *= alpha[rr];
+        }
+#pragma unroll
+        for (int i = 0; i < 32; ++i) o[i] *= alpha[(i >> 1) & 1];
+        const float moff0 = (m_used[0] == -INFINITY) ? 0.f : m_used[0] * p.sl2;
+        const float moff1 = (m_used[1] == -INFINITY) ? 0.f : m_used[1] * p.sl2;
+        // P in the A-operand fragment order: k-step kk covers keys 16 kk .. 16 kk + 15 = score blocks 2 kk, 2 kk + 1
+        uint32_t pa[SW / 16][4];
+#pragma unroll
+        for (int nb = 0; nb < SW / 8; ++nb) {
+          const float a0 = ex2(fmaf(s[nb * 4], p.sl2, -moff0)), a1 = ex2(fmaf(s[nb * 4 + 1], p.sl2, -moff0));
+          const float a2 = ex2(fmaf(s[nb * 4 + 2], p.sl2, -moff1)), a3 = ex2(fmaf(s[nb * 4 + 3], p.sl2, -moff1));
+          l_run[0] += a0 + a1;
+          l_run[1] += a2 + a3;
+          pa[nb >> 1][(nb & 1) * 2] = packp<BF16>(a0, a1);
+          pa[nb >> 1][(nb & 1) * 2 + 1] = packp<BF16>(a2, a3);
+        }
+        if (hh == 0) mbar_wait(&v_full[st], ph);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < SW / 16; ++kk) {
+          // A = {rows fr: keys 16kk + fc.., rows fr+8: same, rows fr: keys 16kk + 8 + fc.., rows fr+8: same}
+          const uint32_t a[4] = {pa[kk][0], pa[kk][1], pa[kk][2], pa[kk][3]};
+          WgmmaRS<BF16>::n64_tb(o, a, vdesc + (uint64_t)((hh * SW + kk * 16) * 128 >> 4));
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        reg_fence(o);
+        if (hh == CS - 1 && wl == 0 && lane == 0) mbar_arrive(&v_empty[st]);
+      }
     }
-    M3R_TR(if (tr) tr[4] = gtime_ns();)
+  }
+  M3R_TR(if (tr) tr[4] = gtime_ns();)
+#pragma unroll
+  for (int rr = 0; rr < 2; ++rr) {
+    l_run[rr] += __shfl_xor_sync(0xffffffffu, l_run[rr], 1);
+    l_run[rr] += __shfl_xor_sync(0xffffffffu, l_run[rr], 2);
+  }
 
-    // ---- epilogue: wait for the last P V, normalise, store (each thread: its row, HD / CS of the 64 output columns)
-    constexpr int OC = HD / CS;
-    uint32_t accr[OC];
-    if (j > 0) {
-      mbar_wait(&o_done[x], (j - 1) & 1);      // last P V (every earlier phase was waited for in the loop)
-      tc_fence_after();
+  // ---- O fragments -> shared memory (over the Q / K stages: every consumer has finished its MMAs), then each thread
+  // takes one row and 32 of its 64 columns: the layout of the stores, the split partials and the merge below.
+  asm volatile("bar.sync 1, %0;" ::"n"(CT) : "memory");
+  {
+    float* so = reinterpret_cast<float*>(smem) + x * (AT_BM * OSTR);
 #pragma unroll
-      for (int c = 0; c < OC / 32; ++c) tmem_ld32(o_addr + c * 32, *reinterpret_cast<uint32_t(*)[32]>(&accr[c * 32]));
-      tmem_wait_ld();
-    } else {
-#pragma unroll
-      for (int d = 0; d < OC; ++d) accr[d] = 0u;
+    for (int nb = 0; nb < 8; ++nb) {
+      so[fr * OSTR + nb * 8 + fc] = o[nb * 4]; so[fr * OSTR + nb * 8 + fc + 1] = o[nb * 4 + 1];
+      so[(fr + 8) * OSTR + nb * 8 + fc] = o[nb * 4 + 2]; so[(fr + 8) * OSTR + nb * 8 + fc + 1] = o[nb * 4 + 3];
     }
-    if (CS == 2) {
-      // row sum = sum of the two halves (added in a fixed order so both threads hold the same value); the buffer of the
-      // parity n_tiles & 1 was last read two tiles ago
-      float* e = xq + (n_tiles & 1) * (2 * AT_BM);
-      e[half * AT_BM + row] = l_run;
-      asm volatile("bar.sync %0, %1;" ::"r"(1 + x), "n"(SMT) : "memory");
-      l_run = e[row] + e[AT_BM + row];
+    float2* sml = reinterpret_cast<float2*>(reinterpret_cast<float*>(smem) + QT * AT_BM * OSTR) + x * AT_BM;
+    if ((lane & 3) == 0) { sml[fr] = make_float2(m_used[0], l_run[0]); sml[fr + 8] = make_float2(m_used[1], l_run[1]); }
+  }
+  asm volatile("bar.sync 1, %0;" ::"n"(CT) : "memory");
+  const int row = threadIdx.x & 127;
+  const int half = (threadIdx.x >> 7) & 1;
+  const int q_idx = q0 + x * AT_BM + row;
+  constexpr int OC = HD / 2;
+  float acc[OC];
+  float m_row, l_row;
+  {
+    const float* so = reinterpret_cast<const float*>(smem) + x * (AT_BM * OSTR) + row * OSTR + half * OC;
+#pragma unroll
+    for (int d = 0; d < OC; ++d) acc[d] = so[d];
+    const float2 ml = (reinterpret_cast<const float2*>(reinterpret_cast<const float*>(smem) + QT * AT_BM * OSTR) + x * AT_BM)[row];
+    m_row = ml.x; l_row = ml.y;
+  }
+  if (q_idx < p.Nq && p.splits == 1 && p.exp_o != nullptr) {
+    const long long grow = (long long)b * p.Nq + q_idx;
+    float4* e4 = reinterpret_cast<float4*>(p.exp_o + (grow * p.H + h) * HD + half * OC);
+#pragma unroll
+    for (int t = 0; t < OC / 4; ++t) e4[t] = make_float4(acc[4 * t], acc[4 * t + 1], acc[4 * t + 2], acc[4 * t + 3]);
+    if (half == 0) p.exp_ml[grow * p.H + h] = make_float2(m_row == -INFINITY ? -INFINITY : m_row * p.sl2, l_row);
+  } else if (q_idx < p.Nq && p.splits == 1) {
+    const long long grow = (long long)b * p.Nq + q_idx;
+    const float inv = l_row > 0.f ? 1.0f / l_row : 0.f;
+    uint4* o4 = reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.O) + grow * p.ldo + h * HD + half * OC);
+#pragma unroll
+    for (int t = 0; t < OC / 8; ++t) {
+      uint4 w;
+      w.x = packp<BF16>(acc[8 * t] * inv, acc[8 * t + 1] * inv);
+      w.y = packp<BF16>(acc[8 * t + 2] * inv, acc[8 * t + 3] * inv);
+      w.z = packp<BF16>(acc[8 * t + 4] * inv, acc[8 * t + 5] * inv);
+      w.w = packp<BF16>(acc[8 * t + 6] * inv, acc[8 * t + 7] * inv);
+      o4[t] = w;
     }
-    float acc[OC];
+  }
+  // key-range splits: unnormalised partial (O, m, l) of this CTA.  Layout [split][unit = (b, h, query tile)][16 column
+  // chunks][128 rows] float4 (and [split][unit][128 rows] float2): lanes are consecutive rows, so both these stores and
+  // the merge's loads are fully coalesced 512 B requests.
+  constexpr int CH = 8;                   // float4 column chunks per thread
+  const int n_qtiles = (p.Nq + AT_BM - 1) / AT_BM;
+  const long long unit = ((long long)b * p.H + h) * n_qtiles + (q0 / AT_BM + x);
+  const long long n_units = (long long)gridDim.z / p.splits * p.H * n_qtiles;
+  // (a second query tile entirely past Nq has no unit of its own: it takes no part in the split bookkeeping)
+  if (p.splits > 1 && q0 + x * AT_BM < p.Nq) {
+    float4* o4 = reinterpret_cast<float4*>(p.part_o) + ((long long)split * n_units + unit) * (16 * AT_BM) + (half * CH) * AT_BM + row;
 #pragma unroll
-    for (int d = 0; d < OC; ++d) acc[d] = __uint_as_float(accr[d]);
-    if (q_idx < p.Nq && p.splits == 1 && p.exp_o != nullptr) {
-      const long long grow = (long long)b * p.Nq + q_idx;
-      float4* e4 = reinterpret_cast<float4*>(p.exp_o + (grow * p.H + h) * HD + half * OC);
-#pragma unroll
-      for (int t = 0; t < OC / 4; ++t) e4[t] = make_float4(acc[4 * t], acc[4 * t + 1], acc[4 * t + 2], acc[4 * t + 3]);
-      if (half == 0) p.exp_ml[grow * p.H + h] = make_float2(m_used == -INFINITY ? -INFINITY : m_used * p.sl2, l_run);
-    } else if (q_idx < p.Nq && p.splits == 1) {
-      const long long grow = (long long)b * p.Nq + q_idx;
-      const float inv = l_run > 0.f ? 1.0f / l_run : 0.f;
-      uint4* o4 = reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.O) + grow * p.ldo + h * HD + half * OC);
-#pragma unroll
-      for (int t = 0; t < OC / 8; ++t) {
-        uint4 w;
-        w.x = packp<BF16>(acc[8 * t] * inv, acc[8 * t + 1] * inv);
-        w.y = packp<BF16>(acc[8 * t + 2] * inv, acc[8 * t + 3] * inv);
-        w.z = packp<BF16>(acc[8 * t + 4] * inv, acc[8 * t + 5] * inv);
-        w.w = packp<BF16>(acc[8 * t + 6] * inv, acc[8 * t + 7] * inv);
-        o4[t] = w;
-      }
+    for (int t = 0; t < CH; ++t) o4[t * AT_BM] = make_float4(acc[4 * t], acc[4 * t + 1], acc[4 * t + 2], acc[4 * t + 3]);
+    if (half == 0)
+      reinterpret_cast<float2*>(p.part_ml)[((long long)split * n_units + unit) * AT_BM + row] =
+          make_float2(m_row == -INFINITY ? -INFINITY : m_row * p.sl2, l_row);
+  }
+  M3R_TR(if (tr) tr[5] = gtime_ns();)
+  if (p.splits > 1 && q0 + x * AT_BM < p.Nq) {
+    // ---- merge of the key-range splits by the last CTA to finish this (batch, head, query tile):
+    // out = sum_s O_s 2^(m_s - m) / sum_s l_s 2^(m_s - m).  No extra kernel launch on the one-view-per-step chain.
+    __shared__ int s_last[2];
+    __threadfence();                                              // partials visible device-wide
+    asm volatile("bar.sync %0, 256;" ::"r"(2 + x) : "memory");    // the softmax threads of this query tile
+    int* cnt = p.split_cnt + unit;
+    if (row == 0 && half == 0) {
+      const int prev = atomicAdd(cnt, 1);
+      s_last[x] = (prev == p.splits - 1);
+      if (prev == p.splits - 1) *cnt = 0;                         // self-cleaning for the next launch
     }
-    // key-range splits: unnormalised partial (O, m, l) of this CTA.  Layout [split][unit = (b, h, query tile)][16 column
-    // chunks][128 rows] float4 (and [split][unit][128 rows] float2): lanes are consecutive rows, so both these stores and
-    // the merge's loads are fully coalesced 512 B requests.
-    constexpr int CH = 16 / CS;                   // float4 column chunks per thread
-    const int n_qtiles = (p.Nq + AT_BM - 1) / AT_BM;
-    const long long unit = ((long long)b * p.H + h) * n_qtiles + (q0 / AT_BM + x);
-    const long long n_units = (long long)gridDim.z / p.splits * p.H * n_qtiles;
-    if (p.splits > 1) {
-      float4* o4 = reinterpret_cast<float4*>(p.part_o) + ((long long)split * n_units + unit) * (16 * AT_BM) + (half * CH) * AT_BM + row;
-#pragma unroll
-      for (int t = 0; t < CH; ++t) o4[t * AT_BM] = make_float4(acc[4 * t], acc[4 * t + 1], acc[4 * t + 2], acc[4 * t + 3]);
-      if (half == 0)
-        reinterpret_cast<float2*>(p.part_ml)[((long long)split * n_units + unit) * AT_BM + row] =
-            make_float2(m_used == -INFINITY ? -INFINITY : m_used * p.sl2, l_run);
-    }
-    M3R_TR(if (tr) tr[5] = gtime_ns();)
-    if (p.splits > 1) {
-      // ---- merge of the key-range splits by the last CTA to finish this (batch, head, query tile):
-      // out = sum_s O_s 2^(m_s - m) / sum_s l_s 2^(m_s - m).  No extra kernel launch on the one-view-per-step chain.
-      __shared__ int s_last[2];
-      __threadfence();                                              // partials visible device-wide
-      asm volatile("bar.sync %0, %1;" ::"r"(1 + x), "n"(SMT) : "memory");    // the softmax threads of this query tile
-      int* cnt = p.split_cnt + unit;
-      if (row == 0 && half == 0) {
-        const int prev = atomicAdd(cnt, 1);
-        s_last[x] = (prev == p.splits - 1);
-        if (prev == p.splits - 1) *cnt = 0;                         // self-cleaning for the next launch
-      }
-      asm volatile("bar.sync %0, %1;" ::"r"(1 + x), "n"(SMT) : "memory");
-      if (s_last[x]) {
-        __threadfence();
-        const float2* mlp = reinterpret_cast<const float2*>(p.part_ml) + unit * AT_BM + row;
-        const float4* op = reinterpret_cast<const float4*>(p.part_o) + unit * (16 * AT_BM) + (half * CH) * AT_BM + row;
-        const long long ml_stride = n_units * AT_BM, o_stride = n_units * (16 * AT_BM);
-        float m = -INFINITY;
+    asm volatile("bar.sync %0, 256;" ::"r"(2 + x) : "memory");
+    if (s_last[x]) {
+      __threadfence();
+      const float2* mlp = reinterpret_cast<const float2*>(p.part_ml) + unit * AT_BM + row;
+      const float4* op = reinterpret_cast<const float4*>(p.part_o) + unit * (16 * AT_BM) + (half * CH) * AT_BM + row;
+      const long long ml_stride = n_units * AT_BM, o_stride = n_units * (16 * AT_BM);
+      float m = -INFINITY;
 #pragma unroll 4
-        for (int sp = 0; sp < p.splits; ++sp) m = fmaxf(m, __ldcg(mlp + sp * ml_stride).x);
-        float l = 0.f;
-        const long long grow = (long long)b * p.Nq + q_idx;
-        // 16 columns at a time: 4 splits x 4 float4 loads in flight per thread, few L2 round trips
+      for (int sp = 0; sp < p.splits; ++sp) m = fmaxf(m, __ldcg(mlp + sp * ml_stride).x);
+      float l = 0.f;
+      const long long grow = (long long)b * p.Nq + q_idx;
+      // 16 columns at a time: 4 splits x 4 float4 loads in flight per thread, few L2 round trips
 #pragma unroll 1
-        for (int qd = 0; qd < CH / 4; ++qd) {
-          float a16[16];
+      for (int qd = 0; qd < CH / 4; ++qd) {
+        float a16[16];
 #pragma unroll
-          for (int d = 0; d < 16; ++d) a16[d] = 0.f;
-          for (int sp0 = 0; sp0 < p.splits; sp0 += 4) {
-            float4 v[4][4];
-            float w[4];
+        for (int d = 0; d < 16; ++d) a16[d] = 0.f;
+        for (int sp0 = 0; sp0 < p.splits; sp0 += 4) {
+          float4 v[4][4];
+          float w[4];
 #pragma unroll
-            for (int u = 0; u < 4; ++u) {
-              const int sp = min(sp0 + u, p.splits - 1);
-              const float2 ml = __ldcg(mlp + sp * ml_stride);
-              w[u] = (sp0 + u < p.splits && ml.x != -INFINITY) ? ex2(ml.x - m) : 0.f;
-              if (qd == 0) l += ml.y * w[u];
+          for (int u = 0; u < 4; ++u) {
+            const int sp = min(sp0 + u, p.splits - 1);
+            const float2 ml = __ldcg(mlp + sp * ml_stride);
+            w[u] = (sp0 + u < p.splits && ml.x != -INFINITY) ? ex2(ml.x - m) : 0.f;
+            if (qd == 0) l += ml.y * w[u];
 #pragma unroll
-              for (int t = 0; t < 4; ++t) v[u][t] = __ldcg(op + sp * o_stride + (qd * 4 + t) * AT_BM);
-            }
+            for (int t = 0; t < 4; ++t) v[u][t] = __ldcg(op + sp * o_stride + (qd * 4 + t) * AT_BM);
+          }
 #pragma unroll
-            for (int u = 0; u < 4; ++u) {
+          for (int u = 0; u < 4; ++u) {
 #pragma unroll
-              for (int t = 0; t < 4; ++t) {
-                a16[4 * t] = fmaf(v[u][t].x, w[u], a16[4 * t]); a16[4 * t + 1] = fmaf(v[u][t].y, w[u], a16[4 * t + 1]);
-                a16[4 * t + 2] = fmaf(v[u][t].z, w[u], a16[4 * t + 2]); a16[4 * t + 3] = fmaf(v[u][t].w, w[u], a16[4 * t + 3]);
-              }
+            for (int t = 0; t < 4; ++t) {
+              a16[4 * t] = fmaf(v[u][t].x, w[u], a16[4 * t]); a16[4 * t + 1] = fmaf(v[u][t].y, w[u], a16[4 * t + 1]);
+              a16[4 * t + 2] = fmaf(v[u][t].z, w[u], a16[4 * t + 2]); a16[4 * t + 3] = fmaf(v[u][t].w, w[u], a16[4 * t + 3]);
             }
           }
-          const float inv = l > 0.f ? 1.0f / l : 0.f;      // l is complete after the first pass
-          if (q_idx < p.Nq && p.exp_o != nullptr) {
-            float4* e4 = reinterpret_cast<float4*>(p.exp_o + (grow * p.H + h) * HD + half * OC + qd * 16);
+        }
+        const float inv = l > 0.f ? 1.0f / l : 0.f;      // l is complete after the first pass
+        if (q_idx < p.Nq && p.exp_o != nullptr) {
+          float4* e4 = reinterpret_cast<float4*>(p.exp_o + (grow * p.H + h) * HD + half * OC + qd * 16);
 #pragma unroll
-            for (int t = 0; t < 4; ++t) e4[t] = make_float4(a16[4 * t], a16[4 * t + 1], a16[4 * t + 2], a16[4 * t + 3]);
-            if (half == 0 && qd == 0) p.exp_ml[grow * p.H + h] = make_float2(m, l);
-          } else if (q_idx < p.Nq) {
-            uint4* o4 = reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.O) + grow * p.ldo + h * HD + half * OC + qd * 16);
+          for (int t = 0; t < 4; ++t) e4[t] = make_float4(a16[4 * t], a16[4 * t + 1], a16[4 * t + 2], a16[4 * t + 3]);
+          if (half == 0 && qd == 0) p.exp_ml[grow * p.H + h] = make_float2(m, l);
+        } else if (q_idx < p.Nq) {
+          uint4* o4 = reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.O) + grow * p.ldo + h * HD + half * OC + qd * 16);
 #pragma unroll
-            for (int t = 0; t < 2; ++t) {
-              uint4 wv;
-              wv.x = packp<BF16>(a16[8 * t] * inv, a16[8 * t + 1] * inv);
-              wv.y = packp<BF16>(a16[8 * t + 2] * inv, a16[8 * t + 3] * inv);
-              wv.z = packp<BF16>(a16[8 * t + 4] * inv, a16[8 * t + 5] * inv);
-              wv.w = packp<BF16>(a16[8 * t + 6] * inv, a16[8 * t + 7] * inv);
-              o4[t] = wv;
-            }
+          for (int t = 0; t < 2; ++t) {
+            uint4 wv;
+            wv.x = packp<BF16>(a16[8 * t] * inv, a16[8 * t + 1] * inv);
+            wv.y = packp<BF16>(a16[8 * t + 2] * inv, a16[8 * t + 3] * inv);
+            wv.z = packp<BF16>(a16[8 * t + 4] * inv, a16[8 * t + 5] * inv);
+            wv.w = packp<BF16>(a16[8 * t + 6] * inv, a16[8 * t + 7] * inv);
+            o4[t] = wv;
           }
         }
       }
     }
   }
-
-  M3R_TR(if (p.trace && threadIdx.x == 0)
-           p.trace[128ull * ((blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) + 6] = gtime_ns();)
-  tc_fence_before();
-  __syncthreads();
-  if (warp == MMA_WARP) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-  }
+M3R_TR(if (p.trace && threadIdx.x == 0)
+         p.trace[128ull * ((blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) + 6] = gtime_ns();)
 }
 
-template <bool BF16, int QT, int POLY, int CS>
+template <bool BF16, int QT, int CS>
 static int launch_attn(const CUtensorMap& tmQ, const CUtensorMap& tmK0, const CUtensorMap& tmV0, const CUtensorMap& tmK1,
                        const CUtensorMap& tmV1, const AttnParams& p, int B, cudaStream_t s) {
-  using Cfg = AttnCfg<QT, CS>;
+  using Cfg = AttnCfg<QT>;
   static bool attr_set[64] = {};               // per device (function attributes are per context)
   int dev = 0; cudaGetDevice(&dev);
   if (dev >= 0 && dev < 64 && !attr_set[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(attn_kernel<BF16, QT, POLY, CS>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
+    cudaError_t e = cudaFuncSetAttribute(attn_kernel<BF16, QT, CS>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
     if (e != cudaSuccess) return set_error("attention: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     attr_set[dev] = true;
   }
   dim3 grid((p.Nq + QT * AT_BM - 1) / (QT * AT_BM), p.H, B * p.splits);
-  cudaError_t e = launch_pdl(attn_kernel<BF16, QT, POLY, CS>, grid, dim3(Cfg::THREADS), Cfg::SMEM, s, tmQ, tmK0, tmV0, tmK1, tmV1, p);
+  cudaError_t e = launch_pdl(attn_kernel<BF16, QT, CS>, grid, dim3(Cfg::THREADS), Cfg::SMEM, s, tmQ, tmK0, tmV0, tmK1, tmV1, p);
   if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) return set_error("attention launch: %s", cudaGetErrorString(e));
   count_launch();
@@ -631,8 +491,8 @@ extern "C" int m3r_attention(const m3r_attn_args* a, void* stream) {
     if (mk3(&tmV1, a->V1, a->ldk1, a->Nk1, a->kv_bstride1, Bkv)) return 1;
   } else { tmK1 = tmK0; tmV1 = tmV0; }
 
-  // ---- shape heuristics (tools/prof_attn.py `sweep` / `longmem`, profiles/r01_attention_variants.txt, profiles/r02_run1_baselines_refgpu_parity.log):
-  //  * enough work for ~half a wave of 2-tile CTAs -> QT=2 (K/V tiles shared by two query tiles, ping-pong), no split;
+  // ---- shape heuristics (tools/prof_attn.py `sweep` / `longmem` compares the variants on a given GPU):
+  //  * enough work for ~half a wave of 2-tile CTAs -> QT=2 (K/V tiles shared by two query tiles), no split;
   //  * otherwise (one view per step) QT=1, two CTAs per SM, and the key range split so that ~2 CTAs per SM exist,
   //    keeping at least 4 key tiles per split; the last CTA of a (batch, head, tile) to finish merges the partials.
   const int sms = num_sms();
@@ -641,15 +501,15 @@ extern "C" int m3r_attention(const m3r_attn_args* a, void* stream) {
   const int ctas1 = ((a->Nq + 127) / 128) * a->H * a->B;
   int qt = (a->Nq > 128 && 2 * ctas2 >= sms) ? 2 : 1;
   //  * one view against a LONG memory (>= ~64 views): two query tiles per CTA halve the K/V bytes each SM pulls per flop,
-  //    which is what bounds the QT=1 form there; the key range is split to fill the SMs (profiles/r02_run1_*: M=100 views
-  //    257 -> 239 us, M=200 497 -> 452 us; below ~50 views QT=1 with splits stays ahead)
+  //    which is what bounds the QT=1 form there; the key range is split to fill the SMs (below ~50 views QT=1 with
+  //    splits stays ahead)
   const bool long_keys = qt == 1 && a->Nq > 128 && key_tiles >= 384 && ctas2 < sms;
   if (long_keys) qt = 2;
   if (const char* f = getenv("M3R_ATTN_QT")) { const int v = atoi(f); if (v == 1 || v == 2) qt = v; }
   int splits = 1;
   if (qt == 1 && ctas1 < 2 * sms) {
     splits = (2 * sms + ctas1 / 2) / ctas1;
-    if (splits > key_tiles / 4) splits = key_tiles / 4;        // a split pays ~2 us of partial store + merge: >= 4 tiles each
+    if (splits > key_tiles / 4) splits = key_tiles / 4;        // a split pays a partial store + merge: >= 4 tiles each
   } else if (qt == 2 && long_keys) {
     splits = (sms + ctas2 / 2) / ctas2;
   } else if (qt == 2 && key_tiles >= 64) {
@@ -703,23 +563,13 @@ extern "C" int m3r_attention(const m3r_attn_args* a, void* stream) {
     const double nk_eff = (double)(a->Nk0 + a->Nk1 - a->skip_len);
     ProfScope prof(qt == 2 ? PROF_ATTN_QT2 : PROF_ATTN_QT1, 4.0 * a->B * (double)a->H * a->Nq * nk_eff * HD,
                    2.0 * ((double)a->B * a->Nq * a->H * HD * 2 + (double)Bkv * (a->Nk0 + a->Nk1) * a->H * HD * 2), cs);
-    // Number of exponential pairs (out of every 8) evaluated by the polynomial instead of the MUFU.  Measured on B200 in
-    // one run (profiles/r01_attention_variants.txt): 0 -> 988 us, 1 -> 917 us, 2 -> 1082 us, 3 -> slower still
-    // (the softmax warps become issue-bound); 1 of 8 is the shipped default.
-    static int poly = -1;
-    if (poly < 0) { const char* e = getenv("M3R_ATTN_POLY"); poly = e ? atoi(e) : 1; if (poly < 0 || poly > 3) poly = 1; }
-    // softmax warpgroups per query tile (column split).  Measured (profiles/r01_attention_variants.txt, run 27): CS=2 is 10 %
-    // slower on the render shape and equal on the one-view shapes (the softmax is issue-bound, not latency-bound: the extra
-    // max exchange + barrier per tile costs more than the added warps hide) -> 1 by default, M3R_ATTN_CS=2 selects it
-    int colsplit = 1;
-    if (const char* e = getenv("M3R_ATTN_CS")) { if (atoi(e) == 2) colsplit = 2; }
+    // score-tile column slices per softmax pass: 2 (default) = two 64-key passes per 128-key tile, half the score
+    // registers; 1 = one 128-key pass (M3R_ATTN_CS=1), which spills at the register budget of two CTAs per SM
+    int colsplit = 2;
+    if (const char* e = getenv("M3R_ATTN_CS")) { if (atoi(e) == 1) colsplit = 1; }
     int rc;
-#define M3R_LAUNCH_ATTN(BF, QTV) (colsplit == 2 ? (poly == 0 ? launch_attn<BF, QTV, 0, 2>(tmQ, tmK0, tmV0, tmK1, tmV1, p, a->B, cs) \
-                                                       : launch_attn<BF, QTV, 1, 2>(tmQ, tmK0, tmV0, tmK1, tmV1, p, a->B, cs)) \
-                                  : poly == 0 ? launch_attn<BF, QTV, 0, 1>(tmQ, tmK0, tmV0, tmK1, tmV1, p, a->B, cs) \
-                                  : poly == 1 ? launch_attn<BF, QTV, 1, 1>(tmQ, tmK0, tmV0, tmK1, tmV1, p, a->B, cs) \
-                                  : poly == 2 ? launch_attn<BF, QTV, 2, 1>(tmQ, tmK0, tmV0, tmK1, tmV1, p, a->B, cs) \
-                                              : launch_attn<BF, QTV, 3, 1>(tmQ, tmK0, tmV0, tmK1, tmV1, p, a->B, cs))
+#define M3R_LAUNCH_ATTN(BF, QTV) (colsplit == 1 ? launch_attn<BF, QTV, 1>(tmQ, tmK0, tmV0, tmK1, tmV1, p, a->B, cs) \
+                                                : launch_attn<BF, QTV, 2>(tmQ, tmK0, tmV0, tmK1, tmV1, p, a->B, cs))
     if (a->is_bf16) rc = qt == 2 ? M3R_LAUNCH_ATTN(true, 2) : M3R_LAUNCH_ATTN(true, 1);
     else rc = qt == 2 ? M3R_LAUNCH_ATTN(false, 2) : M3R_LAUNCH_ATTN(false, 1);
 #undef M3R_LAUNCH_ATTN

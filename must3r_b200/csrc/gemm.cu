@@ -1,11 +1,11 @@
-// Persistent warp-specialised tcgen05 GEMM for sm_100a:  out = epilogue(A[M,K] * W[N,K]^T).
+// Persistent warp-specialised wgmma GEMM for sm_90a:  out = epilogue(A[M,K] * W[N,K]^T).
 //
-//   warp 0      : TMA producer (one elected lane) -- A and W tiles, 128B-swizzled, mbarrier ring
-//   warp 1      : TMEM allocator + single-thread tcgen05.mma issuer (128 x BN x 16 per instruction)
-//   warps 2..9  : epilogue -- tcgen05.ld the fp32 accumulator (one row per thread, half the columns per warp), bias / RoPE / GELU /
-//                 residual / image2-embed row bias, vectorised global stores
-// The accumulator is double-buffered in TMEM (2 x BN columns) so the epilogue of tile i overlaps the MMAs of
-// tile i+1.  Tiles are walked m-fastest so that co-resident CTAs share the weight tile in L2.
+//   warps 0..7 : two consumer warpgroups -- warpgroup w multiplies rows [64w, 64w + 64) of the 128-row tile with
+//                wgmma.m64nBNk16 (operands straight from the 128B-swizzled smem ring, fp32 accumulator in registers),
+//                then runs the epilogue: bias / RoPE / GELU / residual / image2-embed row bias, vectorised global stores
+//   warp 8     : TMA producer (one elected lane) -- A and W tiles, 128B-swizzled, mbarrier ring
+// The producer keeps filling the ring for the next tile while the consumers drain the current one.  Tiles are walked
+// m-fastest so that co-resident CTAs share the weight tile in L2.
 #include <map>
 #include <mutex>
 #include <utility>
@@ -16,19 +16,19 @@ namespace m3r {
 
 constexpr int BM = 128;
 constexpr int BK = 64;        // 64 x 16-bit = 128 B = one swizzle atom
-constexpr int UMMA_K = 16;
-constexpr int GEMM_THREADS = 320;      // TMA warp, MMA warp, 8 epilogue warps (2 per TMEM lane quarter, half the columns each)
-constexpr int SMEM_BUDGET = 196608;  // bytes of operand ring
+constexpr int MMA_K = 16;
+constexpr int GEMM_THREADS = 288;      // 2 consumer warpgroups + the TMA warp
+constexpr int PRODUCER_WARP = 8;
+constexpr int SMEM_MAX = 232448;       // 227 KB: the most dynamic shared memory an sm_90 block may opt in to
 
 template <int BN>
 struct GemmCfg {
   static constexpr int STAGE_BYTES = (BM + BN) * BK * 2;
-  static constexpr int STAGES = SMEM_BUDGET / STAGE_BYTES;   // 256:4  192:4  160:5  128:6  64:8
-  static constexpr int TMEM_COLS = 2 * BN <= 32 ? 32 : 2 * BN <= 64 ? 64 : 2 * BN <= 128 ? 128 : 2 * BN <= 256 ? 256 : 512;   // power of two
-  static constexpr int NCHUNK = BN / 32;                     // 32-column epilogue chunks
-  static constexpr int CH0 = (NCHUNK + 1) / 2;               // chunks drained by the first warp of a lane quarter; the second takes the rest
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
-  static constexpr int PEER_STAGE_BYTES = 8 * 4096;          // per epilogue warp 32 rows x 128 B: transposes peer stores (below)
+  static constexpr int STG_BYTES = 2 * 2 * 64 * 33 * 4;        // epilogue transpose: [warpgroup][chunk][64 rows][33]
+  static constexpr int PEER_STAGE_BYTES = 8 * 4096;          // per consumer warp 32 rows x 128 B: transposes peer stores (below)
+  static constexpr int FIXED = 1024 /*align*/ + 256 /*barriers*/ + STG_BYTES + PEER_STAGE_BYTES;
+  static constexpr int STAGES = (SMEM_MAX - FIXED) / STAGE_BYTES;   // 256:3  192:4  160:4  128:5  64:6  32:8
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256 + STG_BYTES;
   static constexpr int SMEM_BYTES_PEER = SMEM_BYTES + PEER_STAGE_BYTES;
 };
 
@@ -132,7 +132,7 @@ __device__ __forceinline__ void epilogue_math(const GemmParams& p, const float* 
 
 // Store of one chunk: fp32 or 16-bit row segment; the 16-bit form optionally also goes to the peers' buffers.
 // A peer store instruction of a warp covers 32 rows x 16 B; the four uint4 of a thread complete a 64-byte segment per
-// row back to back, so NVLink sees 64 B write bursts (the fused GEMM -> all-gather path, DESIGN.md section 5).
+// row back to back, so NVLink sees 64 B write bursts (the fused GEMM -> all-gather path).
 __device__ __forceinline__ void epilogue_store(const GemmParams& p, void* out, void* const* peers, const float (&v)[32], long long orow, int col0) {
   if (p.out_dtype == 0) {
     float4* o4 = reinterpret_cast<float4*>(reinterpret_cast<float*>(out) + orow * p.ldc + col0);
@@ -187,6 +187,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             const __grid_constant__ typename TabOf<MODE>::type tab) {
   using Cfg = GemmCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
+  constexpr int NCHUNK = BN / 32;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;                               // STAGES x [128 x 64] 16-bit
@@ -194,9 +195,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
   uint64_t* full = bars;                  // [STAGES]
   uint64_t* empty = bars + STAGES;        // [STAGES]
-  uint64_t* tfull = bars + 2 * STAGES;    // [2]
-  uint64_t* tempty = bars + 2 * STAGES + 2;  // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
+  float* stg_all = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES + 256);    // [2 warpgroups][2 chunks][64][33]
 
   M3R_TR(unsigned long long* tr = p.trace ? p.trace + 16ull * blockIdx.x : nullptr;
          if (tr && threadIdx.x == 0) { tr[0] = gtime_ns(); tr[8] = smid(); })
@@ -217,24 +216,16 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   auto a_row0 = [&](int tm) { return (tm / tiles_mg) * p.M + (tm % tiles_mg) * BM; };      // first A row of m-tile tm
   auto w_row0 = [&](int tm, int tn) { return (long long)(tm / tiles_mg) * p.w_group_rows + (long long)tn * BN; };
 
-  if (warp == 0 && elect_one()) {
+  if (warp == PRODUCER_WARP && elect_one()) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmW);
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tfull[s], 1); mbar_init(&tempty[s], 256); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }   // empty: one arrival per warpgroup
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   M3R_TR(if (tr && threadIdx.x == 0) tr[1] = gtime_ns();)
 
-  if (warp == 0) {
+  if (warp == PRODUCER_WARP) {
     // ------------------------------------------------------------ TMA producer
     if (elect_one()) {
       // The weights never depend on the kernel before this one, so the W halves of the first ring of stages are requested
@@ -274,231 +265,236 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       griddep_wait();
       griddep_launch();
     }
-  } else if (warp == 1) {
-    griddep_wait();        // everything above overlapped the previous kernel's tail
-    griddep_launch();
-    // ------------------------------------------------------------ MMA issuer
-    const uint32_t idesc = make_idesc(BM, BN, p.is_bf16 ? 1u : 0u, 0, 0);
-    int stage = 0; uint32_t phase = 0;
-    int as = 0; uint32_t aphase = 0;
-    for (int t = tile0; t < num_tiles; t += tile_step) {
-      mbar_wait(&tempty[as], aphase ^ 1);      // epilogue has drained this accumulator buffer
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + as * BN;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full[stage], phase);
-        M3R_TR(if (tr && kb == 0 && t == tile0 && (threadIdx.x & 31) == 0) tr[4] = gtime_ns();)
-        tc_fence_after();
-        if (elect_one()) {
-          const uint64_t adesc = smem_desc_sw128(smem_u32(sA + stage * BM * BK * 2));
-          const uint64_t bdesc = smem_desc_sw128(smem_u32(sB + stage * BN * BK * 2));
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) {
-            // advance 16 elements (32 bytes) along K inside the 128B swizzle atom: +2 in the >>4 address field
-            umma_ss(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) ? 1u : 0u);
-          }
-          umma_commit(&empty[stage]);                       // frees the smem stage when the MMAs retire
-          if (kb == num_kb - 1) umma_commit(&tfull[as]);    // accumulator complete
-          M3R_TR(if (tr && kb == num_kb - 1) tr[5] = gtime_ns();)
-        }
-        __syncwarp();
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      if (++as == 2) { as = 0; aphase ^= 1; }
-    }
-  } else {
-    // ------------------------------------------------------------ epilogue warps (2..9)
-    griddep_wait();
-    griddep_launch();
-    const int quarter = warp & 3;                 // TMEM lane quarter this warp may access
-    const int chalf = (warp - 2) >> 2;            // which share of the tile's 32-column chunks this warp drains
-    const int c_lo = chalf == 0 ? 0 : Cfg::CH0, c_hi = chalf == 0 ? Cfg::CH0 : Cfg::NCHUNK;
-    const int lane = threadIdx.x & 31;
-    int as = 0; uint32_t aphase = 0;
-    for (int t = tile0; t < num_tiles; t += tile_step) {
-      const int tm = t % tiles_m, tn = t / tiles_m;
-      const int g = tm / tiles_mg;
-      const int lrow = (tm % tiles_mg) * BM + quarter * 32 + lane;      // row inside the group
-      const int n0 = tn * BN;
-      const bool row_ok = lrow < p.M;
-      long long orow = lrow;
-      if (p.rows_per_batch > 0) orow = (long long)(lrow / p.rows_per_batch) * p.batch_stride_rows + lrow % p.rows_per_batch;
-      const bool rb_on = p.rowbias != nullptr && (lrow % p.rb_period) >= p.rb_first;
-      const float* rope_row = p.rope_tab ? p.rope_tab + (long long)(lrow % p.rope_period) * 64 : nullptr;
-      const float* bias = p.bias ? p.bias + (long long)g * p.bias_group : nullptr;
+    return;
+  }
 
-      mbar_wait(&tfull[as], aphase);
-      M3R_TR(if (tr && threadIdx.x == 64) tr[6] = gtime_ns();)
-      tc_fence_after();
-      const uint32_t t_addr = tmem_base + (uint32_t(quarter * 32) << 16) + as * BN;
-      if (MODE == MODE_EMIT) {
-        // ---- x = acc + bias + residual -> out (fp32); the thread keeps its BN/2 values for the normalisation
-        static_assert(MODE != MODE_EMIT || BN == 64, "LayerNorm-emitting epilogue: one 32-column chunk per thread");
-        uint32_t raw[32];
-        tmem_ld32(t_addr + c_lo * 32, raw);
-        tmem_wait_ld();
-        tc_fence_before();
-        mbar_arrive(&tempty[as]);
-        if (ksplit > 1) {
-          // [tile][column half][8 float4][128 rows]: lanes are consecutive rows -> 512 B per warp request
-          float4* kp = p.kpart + ((long long)(t * 2 + chalf) * 8) * BM + (quarter * 32 + lane);
-          if (ks == 1) {
+  // ------------------------------------------------------------ consumer warpgroups 0, 1: wgmma + epilogue
+  griddep_wait();
+  griddep_launch();
+  const int wg = warp >> 2;                       // rows [64 wg, 64 wg + 64) of the tile
+  const int ct = threadIdx.x & 127;
+  const int wl = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const int u = ct >> 6;                          // epilogue: which chunk of a pair this thread drains ...
+  const int r = ct & 63;                          // ... for which row of the warpgroup's 64
+  float* stg = stg_all + wg * (2 * 64 * 33);
+  int stage = 0; uint32_t phase = 0;
+  for (int t = tile0; t < num_tiles; t += tile_step) {
+    const int tm = t % tiles_m, tn = t / tiles_m;
+    const int g = tm / tiles_mg;
+    float acc[BN / 2];
 #pragma unroll
-            for (int i = 0; i < 8; ++i)
-              kp[(long long)i * BM] = make_float4(__uint_as_float(raw[4 * i]), __uint_as_float(raw[4 * i + 1]), __uint_as_float(raw[4 * i + 2]), __uint_as_float(raw[4 * i + 3]));
-            __threadfence();
-            asm volatile("bar.sync 1, 256;" ::: "memory");
-            if (warp == 2 && lane == 0) atom_add_release_u32(p.kflag + t, 1u);
-            continue;                                           // the partner CTA finishes the tile
-          }
-          if (warp == 2 && lane == 0) {
-            unsigned int spins = 0;
-            while (ld_acquire_u32(p.kflag + t) == 0u) { if (++spins > (1u << 26)) __trap(); }
-            p.kflag[t] = 0u;                                    // re-armed for the next launch (nobody else touches it any more)
-          }
-          asm volatile("bar.sync 1, 256;" ::: "memory");
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int prev = -1;
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait(&full[stage], phase);
+      M3R_TR(if (tr && kb == 0 && t == tile0 && threadIdx.x == 0) tr[4] = gtime_ns();)
+      const uint64_t adesc = smem_desc_sw128(smem_u32(sA + stage * BM * BK * 2 + wg * 64 * 128));
+      const uint64_t bdesc = smem_desc_sw128(smem_u32(sB + stage * BN * BK * 2));
+      wgmma_fence();
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float4 o = __ldcg(kp + (long long)i * BM);
-            raw[4 * i] = __float_as_uint(__uint_as_float(raw[4 * i]) + o.x); raw[4 * i + 1] = __float_as_uint(__uint_as_float(raw[4 * i + 1]) + o.y);
-            raw[4 * i + 2] = __float_as_uint(__uint_as_float(raw[4 * i + 2]) + o.z); raw[4 * i + 3] = __float_as_uint(__uint_as_float(raw[4 * i + 3]) + o.w);
+      for (int k = 0; k < BK / MMA_K; ++k) {
+        // advance 16 elements (32 bytes) along K inside the 128B swizzle atom: +2 in the >>4 address field
+        if (p.is_bf16) Wgmma<BN, true>::ss(acc, adesc + 2 * k, bdesc + 2 * k, 1);
+        else Wgmma<BN, false>::ss(acc, adesc + 2 * k, bdesc + 2 * k, 1);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();                            // the previous k-block's MMAs are done: its stage may be refilled
+      reg_fence(acc);
+      if (prev >= 0 && ct == 0) mbar_arrive(&empty[prev]);
+      prev = stage;
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    reg_fence(acc);
+    if (prev >= 0 && ct == 0) mbar_arrive(&empty[prev]);
+    M3R_TR(if (tr && threadIdx.x == 0) tr[5] = gtime_ns();)
+
+    const int lrow = (tm % tiles_mg) * BM + wg * 64 + r;              // row inside the group
+    const int n0 = tn * BN;
+    const bool row_ok = lrow < p.M;
+    long long orow = lrow;
+    if (p.rows_per_batch > 0) orow = (long long)(lrow / p.rows_per_batch) * p.batch_stride_rows + lrow % p.rows_per_batch;
+    const bool rb_on = p.rowbias != nullptr && (lrow % p.rb_period) >= p.rb_first;
+    const float* rope_row = p.rope_tab ? p.rope_tab + (long long)(lrow % p.rope_period) * 64 : nullptr;
+    const float* bias = p.bias ? p.bias + (long long)g * p.bias_group : nullptr;
+    void* out_g = p.out;
+    void* const* peers_g = p.peer_out;
+    if constexpr (MODE == MODE_GROUPED) { out_g = tab.out[g]; peers_g = tab.peer[g]; }
+
+    // The accumulator fragments are transposed through shared memory two 32-column chunks at a time, so that each
+    // epilogue thread owns 32 consecutive columns of ONE row (the layout the bias / RoPE / LayerNorm code works on):
+    // chunks c and c + 1 of the warpgroup's 64 rows go to smem, thread (u, r) reads back row r of chunk c + u.
+    auto stage_pair = [&](int c, uint32_t (&raw)[32]) {
+      asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");        // the previous pair has been read
+#pragma unroll
+      for (int uu = 0; uu < 2; ++uu) {
+        if (c + uu < NCHUNK) {
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) {
+            const int nb = (c + uu) * 4 + jj;
+            float* s0 = stg + uu * (64 * 33) + (wl * 16 + (lane >> 2)) * 33 + jj * 8 + 2 * (lane & 3);
+            s0[0] = acc[nb * 4]; s0[1] = acc[nb * 4 + 1];
+            s0[8 * 33] = acc[nb * 4 + 2]; s0[8 * 33 + 1] = acc[nb * 4 + 3];
           }
         }
-        float v[32];
-        epilogue_math(p, bias, raw, v, lrow, row_ok, rb_on, rope_row, n0 + c_lo * 32);
+      }
+      asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+      if (c + u < NCHUNK) {
+        const float* s1 = stg + u * (64 * 33) + r * 33;
+#pragma unroll
+        for (int i = 0; i < 32; ++i) raw[i] = __float_as_uint(s1[i]);
+      }
+    };
+    if constexpr (MODE == MODE_EMIT) {
+      // ---- x = acc + bias + residual -> out (fp32); the thread keeps its values (chunks u, u + 2, ...) for the normalisation
+      constexpr int CPT = BN / 64;                                 // 32-column chunks per thread
+      uint32_t rawc[CPT][32];
+#pragma unroll
+      for (int pi = 0; pi < CPT; ++pi) stage_pair(2 * pi, rawc[pi]);
+      const int rit = wg * 64 + r;                                 // row in tile
+      if (ksplit > 1) {                                            // BN == 64 only (host)
+        // [tile][column chunk][8 float4][128 rows]: lanes are consecutive rows -> 512 B per warp request
+        uint32_t (&raw)[32] = rawc[0];
+        float4* kp = p.kpart + ((long long)(t * NCHUNK + u) * 8) * BM + rit;
+        if (ks == 1) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i)
+            kp[(long long)i * BM] = make_float4(__uint_as_float(raw[4 * i]), __uint_as_float(raw[4 * i + 1]), __uint_as_float(raw[4 * i + 2]), __uint_as_float(raw[4 * i + 3]));
+          __threadfence();
+          asm volatile("bar.sync 1, 256;" ::: "memory");
+          if (threadIdx.x == 0) atom_add_release_u32(p.kflag + t, 1u);
+          continue;                                           // the partner CTA finishes the tile
+        }
+        if (threadIdx.x == 0) {
+          unsigned int spins = 0;
+          while (ld_acquire_u32(p.kflag + t) == 0u) { if (++spins > (1u << 26)) __trap(); }
+          p.kflag[t] = 0u;                                    // re-armed for the next launch (nobody else touches it any more)
+        }
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const float4 o = __ldcg(kp + (long long)i * BM);
+          raw[4 * i] = __float_as_uint(__uint_as_float(raw[4 * i]) + o.x); raw[4 * i + 1] = __float_as_uint(__uint_as_float(raw[4 * i + 1]) + o.y);
+          raw[4 * i + 2] = __float_as_uint(__uint_as_float(raw[4 * i + 2]) + o.z); raw[4 * i + 3] = __float_as_uint(__uint_as_float(raw[4 * i + 3]) + o.w);
+        }
+      }
+      const int parts = NCHUNK * tiles_n;                          // 32-column partials per row
+      float2* st = p.stats + ((long long)tm * parts) * BM;
+      float v[CPT][32];
+#pragma unroll
+      for (int pi = 0; pi < CPT; ++pi) {
+        const int cc = 2 * pi + u;
+        epilogue_math(p, bias, rawc[pi], v[pi], lrow, row_ok, rb_on, rope_row, n0 + cc * 32);
         if (!row_ok) {
 #pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = 0.f;
+          for (int i = 0; i < 32; ++i) v[pi][i] = 0.f;
         }
-        // two-pass statistics of the thread's 32 values, combined across the row's 2 * tiles_n partials with Chan's
-        // formula (as accurate as a two-pass LayerNorm over the whole row)
+        // two-pass statistics of the thread's 32 values, combined across the row's partials with Chan's formula (as
+        // accurate as a two-pass LayerNorm over the whole row)
         float s0 = 0.f, s1 = 0.f;
 #pragma unroll
-        for (int i = 0; i < 32; i += 2) { s0 += v[i]; s1 += v[i + 1]; }
+        for (int i = 0; i < 32; i += 2) { s0 += v[pi][i]; s1 += v[pi][i + 1]; }
         const float mu = (s0 + s1) * (1.0f / 32.0f);
         float q0 = 0.f, q1 = 0.f;
 #pragma unroll
-        for (int i = 0; i < 32; i += 2) { const float a = v[i] - mu, b = v[i + 1] - mu; q0 = fmaf(a, a, q0); q1 = fmaf(b, b, q1); }
-        const int parts = 2 * tiles_n;
-        const int rit = quarter * 32 + lane;                       // row in tile
-        float2* st = p.stats + ((long long)tm * parts) * BM;
-        st[(long long)(tn * 2 + chalf) * BM + rit] = make_float2(mu, q0 + q1);
-        __threadfence();
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        unsigned int* cnt = p.sync + 2 * tm;
-        if (warp == 2 && lane == 0) atom_add_release_u32(cnt, 1u);
-        // the fp32 residual stream goes out while the other CTAs of the row block arrive (its 32 KB per CTA would otherwise
-        // sit in front of the fence above)
-        if (row_ok) epilogue_store(p, p.out, p.peer_out, v, orow, n0 + c_lo * 32);
-        if (warp == 2 && lane == 0) {
-          unsigned int spins = 0;
-          while (ld_acquire_u32(cnt) < (unsigned int)tiles_n) { if (++spins > (1u << 26)) __trap(); }
-        }
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        float msum = 0.f;
-        float2 pr[24];
-        const int np = parts <= 24 ? parts : 24;                   // host guarantees parts <= 24
+        for (int i = 0; i < 32; i += 2) { const float a = v[pi][i] - mu, b = v[pi][i + 1] - mu; q0 = fmaf(a, a, q0); q1 = fmaf(b, b, q1); }
+        st[(long long)(tn * NCHUNK + cc) * BM + rit] = make_float2(mu, q0 + q1);
+      }
+      __threadfence();
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      unsigned int* cnt = p.sync + 2 * tm;
+      if (threadIdx.x == 0) atom_add_release_u32(cnt, 1u);
+      // the fp32 residual stream goes out while the other CTAs of the row block arrive (its 32 KB per CTA would otherwise
+      // sit in front of the fence above)
+      if (row_ok) {
 #pragma unroll
-        for (int i = 0; i < 24; ++i) if (i < np) { pr[i] = __ldcg(st + (long long)i * BM + rit); msum += pr[i].x; }
-        const float mean = msum / (float)np;
-        float m2 = 0.f;
+        for (int pi = 0; pi < CPT; ++pi) epilogue_store(p, p.out, p.peer_out, v[pi], orow, n0 + (2 * pi + u) * 32);
+      }
+      if (threadIdx.x == 0) {
+        unsigned int spins = 0;
+        while (ld_acquire_u32(cnt) < (unsigned int)tiles_n) { if (++spins > (1u << 26)) __trap(); }
+      }
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      float msum = 0.f;
+      float2 pr[24];
+      const int np = parts <= 24 ? parts : 24;                   // host guarantees parts <= 24
 #pragma unroll
-        for (int i = 0; i < 24; ++i) if (i < np) { const float d = pr[i].x - mean; m2 += pr[i].y + 32.0f * d * d; }
-        const float rstd = rsqrtf(m2 / (32.0f * (float)np) + p.norm_eps);
-        if (row_ok) {
-          uint4* o4 = reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.norm_out) + (long long)lrow * p.ldn + n0 + c_lo * 32);
+      for (int i = 0; i < 24; ++i) if (i < np) { pr[i] = __ldcg(st + (long long)i * BM + rit); msum += pr[i].x; }
+      const float mean = msum / (float)np;
+      float m2 = 0.f;
+#pragma unroll
+      for (int i = 0; i < 24; ++i) if (i < np) { const float d = pr[i].x - mean; m2 += pr[i].y + 32.0f * d * d; }
+      const float rstd = rsqrtf(m2 / (32.0f * (float)np) + p.norm_eps);
+      if (row_ok) {
+#pragma unroll
+        for (int pi = 0; pi < CPT; ++pi) {
+          uint4* o4 = reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.norm_out) + (long long)lrow * p.ldn + n0 + (2 * pi + u) * 32);
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
             uint4 w;
-            w.x = pack16((v[8 * i] - mean) * rstd, (v[8 * i + 1] - mean) * rstd, p.is_bf16);
-            w.y = pack16((v[8 * i + 2] - mean) * rstd, (v[8 * i + 3] - mean) * rstd, p.is_bf16);
-            w.z = pack16((v[8 * i + 4] - mean) * rstd, (v[8 * i + 5] - mean) * rstd, p.is_bf16);
-            w.w = pack16((v[8 * i + 6] - mean) * rstd, (v[8 * i + 7] - mean) * rstd, p.is_bf16);
+            w.x = pack16((v[pi][8 * i] - mean) * rstd, (v[pi][8 * i + 1] - mean) * rstd, p.is_bf16);
+            w.y = pack16((v[pi][8 * i + 2] - mean) * rstd, (v[pi][8 * i + 3] - mean) * rstd, p.is_bf16);
+            w.z = pack16((v[pi][8 * i + 4] - mean) * rstd, (v[pi][8 * i + 5] - mean) * rstd, p.is_bf16);
+            w.w = pack16((v[pi][8 * i + 6] - mean) * rstd, (v[pi][8 * i + 7] - mean) * rstd, p.is_bf16);
             o4[i] = w;
           }
         }
-        // departure: the last CTA of the m-tile to have read the partials re-arms both counters for the next launch
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (warp == 2 && lane == 0) {
-          if (atomicAdd(cnt + 1, 1u) == (unsigned int)tiles_n - 1u) { cnt[1] = 0u; __threadfence(); cnt[0] = 0u; }
-        }
-      } else {
-        void* out_g = p.out;
-        void* const* peers_g = p.peer_out;
-        if constexpr (MODE == MODE_GROUPED) { out_g = tab.out[g]; peers_g = tab.peer[g]; }
-        if (c_lo == c_hi) {                       // narrow tiles: this warp has no chunk, it only returns the buffer
-          tc_fence_before();
-          mbar_arrive(&tempty[as]);
-        }
-        if (p.n_peer_out > 0 && p.out_dtype != 0) {
-          // ---- fused GEMM -> all-gather epilogue.  A thread owns one ROW of the tile, so direct peer stores would be 32
-          // scattered 16-byte pieces per instruction - partial sectors over NVLink (measured 180 GB/s at 8 GPUs, r02_run6).
-          // The warp's rows x (up to) 64 columns go through a swizzled shared-memory tile and leave as 128-byte row segments:
-          // one store instruction = 4 rows x 128 B (8 lanes per row), full sectors, to every peer's buffer.
-          uint4* stg = reinterpret_cast<uint4*>(smem + STAGES * Cfg::STAGE_BYTES + 256) + (warp - 2) * 256;      // [32 rows][8 x 16 B]
-          const int row_base = (tm % tiles_mg) * BM + quarter * 32;
-#pragma unroll 1
-          for (int c = c_lo; c < c_hi; c += 2) {
-            const int nch = (c_hi - c) < 2 ? (c_hi - c) : 2;
-            for (int u = 0; u < nch; ++u) {
-              uint32_t raw[32];
-              tmem_ld32(t_addr + (c + u) * 32, raw);
-              tmem_wait_ld();
-              if (c + u == c_hi - 1) { tc_fence_before(); mbar_arrive(&tempty[as]); }
-              float v[32];
-              epilogue_math(p, bias, raw, v, lrow, row_ok, rb_on, rope_row, n0 + (c + u) * 32);
-              uint4* o4 = reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(out_g) + orow * p.ldc + n0 + (c + u) * 32);
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                uint4 w;
-                w.x = pack16(v[8 * i], v[8 * i + 1], p.is_bf16); w.y = pack16(v[8 * i + 2], v[8 * i + 3], p.is_bf16);
-                w.z = pack16(v[8 * i + 4], v[8 * i + 5], p.is_bf16); w.w = pack16(v[8 * i + 6], v[8 * i + 7], p.is_bf16);
-                if (row_ok) o4[i] = w;                                  // this GPU's copy: the thread's own row
-                stg[lane * 8 + ((u * 4 + i) ^ (lane & 7))] = w;
-              }
-            }
-            __syncwarp();
-            const int lpr = 4 * nch, rpi = 32 / lpr;                    // lanes per row, rows per store instruction
-            for (int k = 0; k < lpr; ++k) {
-              const int r = k * rpi + lane / lpr, piece = lane % lpr;
-              const int row_r = row_base + r;
-              if (row_r < p.M) {
-                long long orow_r = row_r;
-                if (p.rows_per_batch > 0) orow_r = (long long)(row_r / p.rows_per_batch) * p.batch_stride_rows + row_r % p.rows_per_batch;
-                const uint4 val = stg[r * 8 + (piece ^ (r & 7))];
-                for (int pr = 0; pr < p.n_peer_out; ++pr)
-                  reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(peers_g[pr]) + orow_r * p.ldc + n0 + c * 32)[piece] = val;
-              }
-            }
-            __syncwarp();
-          }
-        } else
-#pragma unroll 1
-        for (int c = c_lo; c < c_hi; ++c) {
-          uint32_t raw[32];
-          tmem_ld32(t_addr + c * 32, raw);
-          tmem_wait_ld();
-          if (c == c_hi - 1) {  // this warp's share of the accumulator is read: hand it back early
-            tc_fence_before();
-            mbar_arrive(&tempty[as]);
-          }
-          float v[32];
-          epilogue_math(p, bias, raw, v, lrow, row_ok, rb_on, rope_row, n0 + c * 32);
-          if (row_ok) epilogue_store(p, out_g, peers_g, v, orow, n0 + c * 32);
-        }
       }
-      M3R_TR(if (tr && threadIdx.x == 64) tr[7] = gtime_ns();)
-      if (++as == 2) { as = 0; aphase ^= 1; }
+      // departure: the last CTA of the m-tile to have read the partials re-arms both counters for the next launch
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      if (threadIdx.x == 0) {
+        if (atomicAdd(cnt + 1, 1u) == (unsigned int)tiles_n - 1u) { cnt[1] = 0u; __threadfence(); cnt[0] = 0u; }
+      }
+      continue;
     }
+#pragma unroll
+    for (int c = 0; c < NCHUNK; c += 2) {
+      uint32_t raw[32];
+      stage_pair(c, raw);
+      const int cc = c + u;                                              // this thread's chunk
+      if (p.n_peer_out > 0 && p.out_dtype != 0) {
+        // ---- fused GEMM -> all-gather epilogue.  A thread owns one ROW of the chunk, so direct peer stores would be 32
+        // scattered 16-byte pieces per instruction - partial sectors over NVLink.  The warp's 32 rows x 32 columns go
+        // through a swizzled shared-memory tile and leave as 64-byte row segments: one store instruction = 8 rows x 64 B
+        // (4 lanes per row), whole sectors, to every peer's buffer.  (u and cc are uniform across a warp.)
+        if (cc < NCHUNK) {
+          uint4* pst = reinterpret_cast<uint4*>(stg_all + 2 * (2 * 64 * 33)) + warp * 256;      // [32 rows][8 x 16 B]
+          const int row_base = (tm % tiles_mg) * BM + wg * 64 + (r & ~31);
+          float v[32];
+          epilogue_math(p, bias, raw, v, lrow, row_ok, rb_on, rope_row, n0 + cc * 32);
+          uint4* o4 = reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(out_g) + orow * p.ldc + n0 + cc * 32);
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            uint4 w;
+            w.x = pack16(v[8 * i], v[8 * i + 1], p.is_bf16); w.y = pack16(v[8 * i + 2], v[8 * i + 3], p.is_bf16);
+            w.z = pack16(v[8 * i + 4], v[8 * i + 5], p.is_bf16); w.w = pack16(v[8 * i + 6], v[8 * i + 7], p.is_bf16);
+            if (row_ok) o4[i] = w;                                  // this GPU's copy: the thread's own row
+            pst[lane * 8 + (i ^ (lane & 7))] = w;
+          }
+          __syncwarp();
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const int rr = k * 8 + lane / 4, piece = lane % 4;
+            const int row_r = row_base + rr;
+            if (row_r < p.M) {
+              long long orow_r = row_r;
+              if (p.rows_per_batch > 0) orow_r = (long long)(row_r / p.rows_per_batch) * p.batch_stride_rows + row_r % p.rows_per_batch;
+              const uint4 val = pst[rr * 8 + (piece ^ (rr & 7))];
+              for (int pr = 0; pr < p.n_peer_out; ++pr)
+                reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(peers_g[pr]) + orow_r * p.ldc + n0 + cc * 32)[piece] = val;
+            }
+          }
+          __syncwarp();
+        }
+      } else if (cc < NCHUNK) {
+        float v[32];
+        epilogue_math(p, bias, raw, v, lrow, row_ok, rb_on, rope_row, n0 + cc * 32);
+        if (row_ok) epilogue_store(p, out_g, peers_g, v, orow, n0 + cc * 32);
+      }
+    }
+    M3R_TR(if (tr && threadIdx.x == 0) tr[7] = gtime_ns();)
   }
-
-  tc_fence_before();
-  __syncthreads();
   M3R_TR(if (tr && threadIdx.x == 0) tr[9] = gtime_ns();)
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-  }
 }
 
 static void fill_params(GemmParams& p, const m3r_gemm_args* a) {
@@ -572,7 +568,7 @@ static int launch_gemm(const m3r_gemm_args* a, cudaStream_t stream, const m3r_ge
     p.norm_out = a->norm_out; p.ldn = a->ldn; p.norm_eps = a->norm_eps; p.stats = e->stats; p.sync = e->sync;
     static int ks_env = -1;
     if (ks_env < 0) { const char* v = getenv("M3R_KSPLIT"); ks_env = (v && v[0] == '0') ? 0 : 1; }
-    if (ks_env && a->K >= 2048 && (a->K / BK) % 2 == 0 && 2 * tiles <= num_sms() && tiles <= EMIT_MAX_KSPLIT_TILES) {
+    if (BN == 64 && ks_env && a->K >= 2048 && (a->K / BK) % 2 == 0 && 2 * tiles <= num_sms() && tiles <= EMIT_MAX_KSPLIT_TILES) {
       p.ksplit = 2; p.kpart = e->kpart; p.kflag = e->kflag;
     }
   }
@@ -596,170 +592,6 @@ static int launch_gemm(const m3r_gemm_args* a, cudaStream_t stream, const m3r_ge
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error("gemm launch: %s", cudaGetErrorString(e));
-  count_launch();
-  return 0;
-}
-
-
-// ------------------------------------------------------------------------------------------------ CTA-pair GEMM
-// Two CTAs of a cluster (the two SMs of a TPC) compute one 256 x 256 output tile with tcgen05.mma.cta_group::2: each
-// CTA stages its own 128 rows of A and HALF of the weight tile (128 of the 256 W rows), so per CTA a k-block costs
-// 32 KB of L2->smem traffic instead of 48 KB and the 192 KB ring holds 6 stages instead of 4 (the 1-CTA kernel's MMA
-// warp spends half its time waiting for operands, profiles/r01_ncu_gemm_v1_summary.txt).  The leader CTA issues the
-// MMAs; completion is multicast to both CTAs' barriers; each CTA's epilogue drains its own 128 accumulator rows.
-constexpr int P_STAGES = 6;
-constexpr int P_STAGE_BYTES = (128 + 128) * BK * 2;          // A rows + half of W per CTA
-constexpr int P_SMEM_BYTES = P_STAGES * P_STAGE_BYTES + 1024 + 256;
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-gemm_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW, const GemmParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sA = smem;                                  // P_STAGES x [128 x 64]
-  uint8_t* sB = smem + P_STAGES * 128 * BK * 2;        // P_STAGES x [128 x 64] (this CTA's half of the W tile)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + P_STAGES * P_STAGE_BYTES);
-  uint64_t* full = bars;                       // [P_STAGES] used in the leader only
-  uint64_t* empty = bars + P_STAGES;           // [P_STAGES] both CTAs (multicast commit)
-  uint64_t* tfull = bars + 2 * P_STAGES;       // [2] both CTAs (multicast commit)
-  uint64_t* tempty = bars + 2 * P_STAGES + 2;  // [2] leader only: 512 arrivals (both CTAs' epilogue threads)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * P_STAGES + 4);
-
-  const int warp = threadIdx.x >> 5;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int tiles_m = (p.M + 255) / 256;
-  const int tiles_n = p.N / 256;
-  const int num_tiles = tiles_m * tiles_n;
-  const int num_kb = p.K / BK;
-  const int pair = blockIdx.x >> 1, n_pairs = gridDim.x >> 1;
-
-  if (warp == 0 && elect_one()) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmW);
-    for (int s = 0; s < P_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tfull[s], 1); mbar_init(&tempty[s], 512); }
-    fence_mbar_init();
-  }
-  if (warp == 1) {
-    tmem_alloc2(tmem_slot, 512);
-    tmem_relinquish2();
-  }
-  tc_fence_before();
-  cluster_sync_all();            // barriers of both CTAs initialised before any remote arrive / TMA signal
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  griddep_wait();
-  griddep_launch();
-
-  if (warp == 0) {
-    // ------------------------------------------------------------ TMA producer (both CTAs)
-    if (elect_one()) {
-      int stage = 0; uint32_t phase = 0;
-      for (int t = pair; t < num_tiles; t += n_pairs) {
-        const int m0 = (t % tiles_m) * 256 + rank * 128;
-        const int n0 = (t / tiles_m) * 256 + rank * 128;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty[stage], phase ^ 1);
-          if (leader) mbar_arrive_expect_tx(&full[stage], 2 * P_STAGE_BYTES);       // bytes of BOTH CTAs
-          const uint32_t lbar = mapa_u32(&full[stage], 0);
-          tma_load_2d_pair(sA + stage * 128 * BK * 2, &tmA, lbar, kb * BK, m0);
-          tma_load_2d_pair(sB + stage * 128 * BK * 2, &tmW, lbar, kb * BK, n0);
-          if (++stage == P_STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------ MMA issuer (leader CTA only)
-    if (leader) {
-      const uint32_t idesc = make_idesc(256, 256, p.is_bf16 ? 1u : 0u, 0, 0);
-      int stage = 0; uint32_t phase = 0;
-      int as = 0; uint32_t aphase = 0;
-      for (int t = pair; t < num_tiles; t += n_pairs) {
-        mbar_wait(&tempty[as], aphase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + as * 256;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          if (elect_one()) {
-            const uint64_t adesc = smem_desc_sw128(smem_u32(sA + stage * 128 * BK * 2));
-            const uint64_t bdesc = smem_desc_sw128(smem_u32(sB + stage * 128 * BK * 2));
-#pragma unroll
-            for (int k = 0; k < BK / UMMA_K; ++k) umma_ss_pair(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) ? 1u : 0u);
-            umma_commit_pair(&empty[stage]);
-            if (kb == num_kb - 1) umma_commit_pair(&tfull[as]);
-          }
-          __syncwarp();
-          if (++stage == P_STAGES) { stage = 0; phase ^= 1; }
-        }
-        if (++as == 2) { as = 0; aphase ^= 1; }
-      }
-    }
-  } else {
-    // ------------------------------------------------------------ epilogue warps (both CTAs, own 128 rows)
-    const int quarter = warp & 3;
-    const int chalf = (warp - 2) >> 2;
-    const int lane = threadIdx.x & 31;
-    int as = 0; uint32_t aphase = 0;
-    const uint32_t tempty_leader[2] = {mapa_u32(&tempty[0], 0), mapa_u32(&tempty[1], 0)};
-    for (int t = pair; t < num_tiles; t += n_pairs) {
-      const int m0 = (t % tiles_m) * 256 + rank * 128;
-      const int n0 = (t / tiles_m) * 256;
-      const int row = m0 + quarter * 32 + lane;
-      const bool row_ok = row < p.M;
-      long long orow = row;
-      if (p.rows_per_batch > 0) orow = (long long)(row / p.rows_per_batch) * p.batch_stride_rows + row % p.rows_per_batch;
-      const bool rb_on = p.rowbias != nullptr && (row % p.rb_period) >= p.rb_first;
-      const float* rope_row = p.rope_tab ? p.rope_tab + (long long)(row % p.rope_period) * 64 : nullptr;
-      mbar_wait(&tfull[as], aphase);
-      tc_fence_after();
-      const uint32_t t_addr = tmem_base + (uint32_t(quarter * 32) << 16) + as * 256;
-#pragma unroll 1
-      for (int c = chalf * 4; c < chalf * 4 + 4; ++c) {
-        uint32_t raw[32];
-        tmem_ld32(t_addr + c * 32, raw);
-        tmem_wait_ld();
-        if (c == chalf * 4 + 3) {
-          tc_fence_before();
-          mbar_arrive_cluster(tempty_leader[as]);
-        }
-        epilogue_chunk(p, raw, row, row_ok, orow, rb_on, rope_row, n0 + c * 32);
-      }
-      if (++as == 2) { as = 0; aphase ^= 1; }
-    }
-  }
-
-  tc_fence_before();
-  cluster_sync_all();            // no CTA leaves (or frees TMEM) while its peer may still address it
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc2(tmem_base, 512);
-  }
-}
-
-static int launch_gemm_pair(const m3r_gemm_args* a, cudaStream_t stream) {
-  CUtensorMap tmA, tmW;
-  if (make_tmap_2d(&tmA, a->A, a->is_bf16, (uint64_t)a->K, (uint64_t)a->M, (uint64_t)a->lda, BK, 128)) return 1;
-  if (make_tmap_2d(&tmW, a->W, a->is_bf16, (uint64_t)a->K, (uint64_t)a->N, (uint64_t)a->ldw, BK, 128)) return 1;
-  GemmParams p;
-  fill_params(p, a);
-  static bool attr_set[64] = {};
-  int dev = 0; cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && !attr_set[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, P_SMEM_BYTES);
-    if (e != cudaSuccess) return set_error("gemm(pair): cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-    attr_set[dev] = true;
-  }
-  const int tiles = ((a->M + 255) / 256) * (a->N / 256);
-  int pairs = num_sms() / 2;
-  if (tiles < pairs) pairs = tiles;
-  {
-    ProfScope prof(PROF_GEMM256, 2.0 * a->M * (double)a->N * a->K, 2.0 * ((double)a->M * a->K + (double)a->N * a->K) + (double)a->M * a->N * (a->out_dtype ? 2 : 4), stream);
-    cudaError_t le = launch_pdl(gemm_pair_kernel, dim3(2 * pairs), dim3(GEMM_THREADS), P_SMEM_BYTES, stream, tmA, tmW, p);
-    if (le != cudaSuccess) return set_error("gemm(pair) launch: %s", cudaGetErrorString(le));
-  }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error("gemm(pair) launch: %s", cudaGetErrorString(e));
   count_launch();
   return 0;
 }
@@ -804,19 +636,12 @@ extern "C" int m3r_gemm(const m3r_gemm_args* a, void* stream) {
     // LayerNorm-emitting epilogue: fp32 out = the new residual stream, norm_out = its normalised 16-bit rows
     if (a->N % 64 || a->N > 32 * EMIT_MAX_PARTS || a->out_dtype != M3R_OUT_F32 || a->ldn % 8)
       return set_error("gemm: norm_out needs N %% 64 == 0, N <= %d, an fp32 output and ldn %% 8 == 0", 32 * EMIT_MAX_PARTS);
+    // every CTA of the launch must be resident at once (they meet at a counter): 128x64 tiles, or 128x128 tiles when the
+    // 64-wide ones would not fit on the SMs in one wave
     const int tiles_m = (a->M + BM - 1) / BM;
-    if (tiles_m > EMIT_MAX_TILES_M || tiles_m * (a->N / 64) > sms)
-      return set_error("gemm: norm_out needs one 128x64 tile per SM (M=%d N=%d); normalise with m3r_layernorm instead", a->M, a->N);
-    return launch_gemm<64, MODE_EMIT>(a, s);
-  }
-  {
-    // CTA-pair kernel for problems with at least one 256x256 tile per SM pair.  Measured (profiles/r01_run13_gemm_pair.log):
-    // +7..+20 % for K >= 1024, -1..-4 % for K = 768 (epilogue-bound tiles) -> used for K >= 1024; M3R_GEMM_PAIR=0/2
-    // force it off / on for every eligible shape.
-    static int pair_mode = -1;
-    if (pair_mode < 0) { const char* e = getenv("M3R_GEMM_PAIR"); pair_mode = e ? atoi(e) : 1; }
-    const bool eligible = a->N % 256 == 0 && ((a->M + 255) / 256) * (a->N / 256) >= sms / 2 && !getenv("M3R_GEMM_BN");
-    if (eligible && (pair_mode == 2 || (pair_mode == 1 && a->K >= 1024))) return launch_gemm_pair(a, s);
+    if (tiles_m <= EMIT_MAX_TILES_M && tiles_m * (a->N / 64) <= sms) return launch_gemm<64, MODE_EMIT>(a, s);
+    if (tiles_m <= EMIT_MAX_TILES_M && a->N % 128 == 0 && tiles_m * (a->N / 128) <= sms) return launch_gemm<128, MODE_EMIT>(a, s);
+    return set_error("gemm: norm_out needs one 128x64 tile per SM (M=%d N=%d); normalise with m3r_layernorm instead", a->M, a->N);
   }
   int bn = pick_bn(a->M, a->N, 1);
   const char* force = getenv("M3R_GEMM_BN");

@@ -51,10 +51,10 @@ ProfScope::~ProfScope() { if (slot >= 0) cudaEventRecord(g_prof[slot].b, stream)
 int num_sms() {
   static int sms[64] = {};                      // per device
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (sms[dev] == 0) {
     cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev);
-    if (sms[dev] <= 0) sms[dev] = 148;
+    if (sms[dev] <= 0) sms[dev] = 132;
   }
   return sms[dev];
 }

@@ -438,7 +438,7 @@ def _ensure_features(encoder, x, pos, imgs, true_shape, lo, hi, max_bs, device):
 # CUDA encoder the missing views are encoded UP FRONT, in large same-shape batches, then the decoder chain runs: measured on
 # C3 63.3 ms vs 88.7 ms for per-step encoding.  (Encoding on a side stream NEXT to the latency-bound chain - SM-capped
 # persistent GEMMs, chain on a high-priority stream - was measured too and lost: 70.5 .. 93.9 ms, the chain's one-wave kernels
-# wait for SMs; profiles/r02_run17_*, r02_run18_*.)  Same kernels, same per-view features (rows are independent).
+# wait for SMs.)  Same kernels, same per-view features (rows are independent).
 ENCODE_AHEAD_BATCH = 50
 
 

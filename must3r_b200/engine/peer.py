@@ -1,6 +1,6 @@
 """Peer-visible device memory for the multi-GPU schedule: buffers allocated by the library (cudaMalloc), exported as CUDA
 IPC handles, exchanged with torch.distributed and mapped by every other rank of the node, so that a GEMM epilogue on one
-GPU can store K|V rows straight into the memory buffers of all GPUs over NVLink (SURVEY.md §8e, DESIGN.md §5)."""
+GPU can store K|V rows straight into the memory buffers of all GPUs over NVLink (SURVEY.md §8e)."""
 from __future__ import annotations
 
 import ctypes as C

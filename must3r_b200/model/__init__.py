@@ -1,5 +1,5 @@
 """Model API of the reference (must3r/model/__init__.py): load_model, Dust3rEncoder, MUSt3R, CausalMUSt3R,
-ActivationType, apply_activation, get_pointmaps_activation, get_dtype - backed by the sm_100a kernels."""
+ActivationType, apply_activation, get_pointmaps_activation, get_dtype - backed by the sm_90a kernels."""
 from __future__ import annotations
 
 import re

@@ -82,7 +82,7 @@ def set_precision(dtype) -> None:
 
     ``torch.float16`` (default): 10-bit mantissa, i.e. the precision class of the TF32 matmuls the
     reference's demos enable (demo.py:12) - the parity mode.  ``torch.bfloat16``: the amp dtype of the
-    reference's decoder (`--amp bf16`).  Both run at the same tcgen05 rate; accumulation, LayerNorm, softmax
+    reference's decoder (`--amp bf16`).  Both run at the same tensor-core rate; accumulation, LayerNorm, softmax
     and the residual stream are fp32 either way."""
     if isinstance(dtype, str):
         dtype = {"fp16": torch.float16, "float16": torch.float16, "bf16": torch.bfloat16, "bfloat16": torch.bfloat16}[dtype]

@@ -1,5 +1,5 @@
 """MUSt3R memory decoder with the reference's constructor, state-dict keys, forward / forward_list
-signatures and memory-tuple format (must3r/model/decoder.py:14-350), executing on the sm_100a kernels.
+signatures and memory-tuple format (must3r/model/decoder.py:14-350), executing on the sm_90a kernels.
 
 Memory tuple (decoder.py:337): ``(list[depth] of Tensor[B,Nmem,2*D], labels int64 [B,Nmem], mem_nimgs,
 mem_protected_imgs, mem_protected_tokens)``.  The K|V tensors are 16-bit (the precision set with

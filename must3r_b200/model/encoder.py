@@ -1,5 +1,5 @@
 """Dust3rEncoder with the reference's constructor, state-dict keys and forward signature
-(must3r/model/encoder.py:13-65), executing on the sm_100a kernels through the C ABI."""
+(must3r/model/encoder.py:13-65), executing on the sm_90a kernels through the C ABI."""
 from __future__ import annotations
 
 import ctypes as C

@@ -283,8 +283,50 @@ def model_args_golden():
     print("model_args.json", len(out["set_image_size"]) + len(out["convert"]), "cases")
 
 
+def keyframe_frame(seed, H=48, W=64, shift=0.0):
+    """Synthetic SLAM frame (same generator as tests/test_keyframes_gpu.py)."""
+    g = torch.Generator().manual_seed(seed)
+    pts = torch.randn(1, 1, H, W, 3, generator=g) * 2.0 + shift
+    loc = pts.clone()
+    loc[..., 2] = loc[..., 2].abs() + 1.0
+    conf = 1.0 + torch.rand(1, 1, H, W, generator=g) * 3.0
+    return {"pts3d": pts, "pts3d_local": loc, "conf": conf}
+
+
+def keyframes_golden():
+    """SLAM keyframe overlap scores of the reference (must3r/slam/model.py get_overlap_score on its scipy KD-tree
+    searchers, must3r/slam/nns.py) and its quadrant ids (must3r/slam/tools.py) -> tests/golden/keyframes.npz."""
+    import must3r.slam.model as slam_model
+    import must3r.slam.nns as nns
+    import must3r.slam.tools as slam_tools
+    out = {}
+    cam = torch.tensor([0.1, -0.2, 0.3])
+    for method in ("kdtree-scipy", "quadrant_x2-kdtree-scipy", "quadrant_x4-kdtree-scipy"):
+        for mode in ("nn", "nn-norm"):
+            tree = nns.get_searcher(method)
+            for i in range(3):
+                fr = keyframe_frame(10 + i, shift=0.5 * i)
+                tree.add_pts(fr["pts3d"][0, 0, ::2, ::2][fr["conf"][0, 0, ::2, ::2] > 1.5], cam_center=cam)
+            for seed, shift in ((50, 0.2), (51, 3.0)):
+                s = slam_model.get_overlap_score(keyframe_frame(seed, shift=shift), tree, cam, mode=mode, kf_x_subsamp=2,
+                                                 min_conf_keyframe=1.5, percentile=70)
+                out[f"{method}.{mode}.{seed}"] = np.array([float(s), float(slam_model.choose_keyframe_from_overlap(s, 0.1, mode))])
+            s = slam_model.get_overlap_score(keyframe_frame(60), nns.get_searcher(method), cam, mode="nn", kf_x_subsamp=2)
+            out[f"{method}.empty"] = np.array([float(s)])
+    fr = keyframe_frame(70)
+    for mode in ("meanconf", "medianconf"):
+        out[mode] = np.array([float(slam_model.get_overlap_score(fr, None, None, mode=mode))])
+    rays = torch.randn(4000, 3, generator=torch.Generator().manual_seed(3))
+    for div in (2, 4):
+        out[f"quadrant{div}"] = np.asarray(slam_tools.get_quadrant_id(rays.clone().numpy(), quadrant_divider=div)).astype(np.int16)
+    np.savez_compressed(os.path.join(HERE, "keyframes.npz"), **out)
+    print("keyframes.npz", len(out), "arrays")
+
+
 if __name__ == "__main__":
     which = sys.argv[1:] or ["tiny", "engine", "full", "args"]
+    if "keyframes" in which:
+        keyframes_golden()
     if "args" in which:
         model_args_golden()
     if "tiny" in which:

@@ -38,7 +38,7 @@ def test_split_and_schedules():
 def test_reference_arm_prints_the_contract_line():
     from baseline import ref_loader
     if not ref_loader.available():
-        pytest.skip("baseline/_ref not installed")
+        pytest.skip("oracle/_ref not installed")
     out = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--impl", "reference", "--config", "c2", "--steps", "1",
                           "--warmup", "1", "--cpu-views", "2"], capture_output=True, text=True, timeout=500)
     assert out.returncode == 0, out.stderr[-2000:]

@@ -1,7 +1,7 @@
 """Model-level parity of the CUDA path (through load_model / Dust3rEncoder / MUSt3R, i.e. the C ABI whole-model
 entry points) against (i) outputs of the unmodified reference (tests/golden/*.npz) and (ii) the CPU oracle.
 
-Tolerances (rel-L2 of raw pointmaps / memory vs the fp32 reference), see DESIGN.md "Numerics":
+Tolerances (rel-L2 of raw pointmaps / memory vs the fp32 reference):
   tiny models (128-wide, 2-3 layers, errors do not average out): fp16 3e-3, bf16 2.5e-2
   full-size models (the benchmarked schedules, test_benchmarked_chains_vs_reference_engine and the 3-view digests):
     fp16 operands 1.0e-3 (1.2e-3 on the 3-view digests' sampled statistics), bf16 1.1e-2 = the reference's own bf16-vs-fp32 gap
@@ -247,7 +247,7 @@ def test_memory_modes_match_kv(mode):
 
 
 # bf16 gate of the full-size chains: the reference's own bf16-autocast-vs-fp32 gap on the raw head output (1.1e-2,
-# BASELINE.md §5 / SURVEY.md §0 fact 10); fp16 operands are the north star's 1e-3 parity mode
+# SURVEY.md §0 fact 10); fp16 operands are the north star's 1e-3 parity mode
 CHAIN_TOL = {torch.float16: 1.0e-3, torch.bfloat16: 1.1e-2}
 # pts3d_local = norm_exp activation of the head's channels 3:6: expm1 amplifies the relative error of the larger |v| of the
 # camera-frame points (measured 1.0e-3 at 224x224, 1.2e-3 at 512x384 with fp16 operands vs 7.7e-4 on the raw head output)

@@ -34,7 +34,9 @@ def _worker(rank, world, port, q, counts=None):
     enc, dec = _models()
     imgs, ts = _views(rank, counts[rank] if counts else V)
     mem, outs = sharded.inference_sharded(enc, dec, imgs, ts, device="cpu", return_mem=True, view_counts=counts)
-    q.put((rank, torch.stack(outs).clone(), [m.clone() for m in mem[0]], mem[1].clone()))
+    # numpy arrays travel by value: torch tensors would be passed as file descriptors that the receiver can only open
+    # while this process is still alive
+    q.put((rank, torch.stack(outs).numpy().copy(), [m.numpy().copy() for m in mem[0]], mem[1].numpy().copy()))
     dist.barrier()
     dist.destroy_process_group()
 
@@ -108,11 +110,16 @@ def test_gloo_matches_composed_oracle(world, counts):
     got = {}
     for _ in range(world):
         r, outs, mem_vals, labels = q.get(timeout=240)
-        got[r] = (outs, mem_vals, labels)
+        got[r] = (torch.from_numpy(outs), [torch.from_numpy(m) for m in mem_vals], torch.from_numpy(labels))
     for p in procs:
         p.join(timeout=60)
         assert p.exitcode == 0
-    mem, renders = _composed_expected(world, counts)
+    threads = torch.get_num_threads()
+    torch.set_num_threads(1)                 # the workers' thread count: same fp32 reduction order on any host
+    try:
+        mem, renders = _composed_expected(world, counts)
+    finally:
+        torch.set_num_threads(threads)
     for r in range(world):
         outs, mem_vals, labels = got[r]
         assert torch.equal(labels, mem[1])                                   # identical memory on every rank

@@ -1,6 +1,6 @@
 """Streaming (video) schedule on one GPU: frames/s of engine.inference_video_multi_ar at 512x384 with the reference's
 defaults (keyframe iff id % 3 == 0, rolling window of 25 frames), with and without the host label shadow that turns
-the engine's memory edits into slice operations (DESIGN.md "Engine memory edits").
+the engine's memory edits into slice operations.
 
     python tools/bench_stream.py [frames=60] [window=25]
 """

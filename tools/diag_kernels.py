@@ -1,4 +1,4 @@
-"""Bring-up diagnostics for the tcgen05 kernels: structured inputs that localise descriptor / layout mistakes.
+"""Bring-up diagnostics for the wgmma kernels: structured inputs that localise descriptor / layout mistakes.
 Prints one line per probe; never asserts.  Run on the GPU box: python tools/diag_kernels.py"""
 import os
 import sys
