@@ -1,22 +1,31 @@
 // FlashAttention-style softmax(Q K^T * scale) V for head_dim 64 on sm_90a tensor cores (wgmma).
 //
-// One CTA = one (batch, head, QT x 128 queries [, key split]).  QT = 2 for throughput shapes: the two query tiles
-// share every K / V tile that TMA brings in (half the L2->smem traffic).  Roles:
-//   warps 0..8*QT-1 : 2*QT consumer warpgroups, 64 query rows each.  Per 128-key tile, in CS column slices (2 x 64 keys by default):
-//                     S[64 x 64] = Q K^T (wgmma, both operands K-major smem, fp32 scores in registers), row max over
-//                     the quad of threads sharing a row, exp2 with the scale folded in, row sums, P packed to 16-bit
+// One CTA = one (batch, head, 128 queries [, key split]), one CTA per SM; the two consumer warpgroups share every K / V
+// tile that TMA brings in.  (A 192-row form with three consumer warpgroups fits only 128 registers per thread: it
+// spills and measured slower on H100.)  Roles:
+//   warpgroup 2     : TMA producer -- Q once, then K and V tiles (128 keys x 64) through mbarrier rings.  It gives its
+//                     registers back (setmaxnreg.dec) so that the consumers can hold two score tiles' worth of state.
+//                     3-D tensor maps: rows beyond Nk read as zeros even inside over-allocated memory buffers.
+//   warpgroups 0, 1 : consumers, 64 query rows each, one whole 128-key tile per pass:
+//                     S[64 x 128] = Q K^T (m64n128 wgmma, both operands K-major smem, fp32 scores in registers), row max
+//                     over the quad of threads sharing a row, exp2 with the scale folded in, row sums, P packed to 16-bit
 //                     straight into the register A operand of O += P V (wgmma with V as an MN-major smem B operand:
 //                     V is consumed in its natural [keys, d] layout -- no transpose anywhere in the pipeline).
-//                     The warpgroups run independently, so one's softmax overlaps another's MMAs.
-//   warp 8*QT       : TMA producer -- Q tiles once, then K and V tiles (128 keys x 64) through mbarrier rings.
-//                     3-D tensor maps: rows beyond Nk read as zeros even inside over-allocated memory buffers.
+//                     Software pipeline inside the warpgroup: S of tile j+1 and O += P V of tile j are issued together,
+//                     and the softmax of tile j+1 runs while P V of tile j is still on the tensor cores.  A K stage is
+//                     released as soon as its scores are in registers, a V stage when its P V has completed.
+//                     (Making the two warpgroups also take turns at the tensor cores through named barriers
+//                     ("ping-pong") measured 1-2 % slower on H100 for the C3 shapes, so they run independently.  With
+//                     every ex2 removed, the render cross-attention ran only 12 % faster: the kernel is not bound by
+//                     the MUFU, and no exponentials are moved to the FMA pipe.)
 // O accumulates in registers across key tiles.  The running max used in the exponent is only refreshed when the true
 // row max grew by more than 2^8 (lazy rescaling); the final O / l is mathematically unchanged.
 //
 // Keys come from two segments (stored memory + this step's new tokens) so the reference's torch.cat of the memory
 // (decoder.py:306) never happens; a per-batch skip range implements make_mem_mask (decoder.py:119-139): fully
 // masked key tiles are never loaded.  Small grids (one view per step) split the key range over several CTAs; the
-// last CTA to finish a (batch, head, query tile) merges the partial (O, m, l) in-kernel.
+// last CTA to finish a (batch, head, 64-row query tile) merges the partial (O, m, l) in-kernel.  The split
+// count comes from a wave-count cost model (m3r_attention).
 #include <math.h>
 #include <map>
 #include <mutex>
@@ -26,21 +35,29 @@
 
 namespace m3r {
 
-constexpr int AT_BM = 128;
+constexpr int AT_BM = 64;                    // query rows per consumer warpgroup: the unit of the epilogue, splits and merge
 constexpr int AT_BN = 128;
 constexpr int HD = 64;
-constexpr int TILE_BYTES = 128 * HD * 2;     // 16 KB
+constexpr int TILE_BYTES = 128 * HD * 2;     // 16 KB: one K or V tile
+constexpr int QTILE_BYTES = AT_BM * HD * 2;  // 8 KB: one warpgroup's Q rows
 constexpr float RESCALE_THRESHOLD = 8.0f;    // log2 units
 
-template <int QT> struct AttnCfg {
-  static constexpr int KS = QT == 2 ? 3 : 2;                       // K / V ring depth
-  static constexpr int THREADS = 32 * (8 * QT + 1);                // consumer warpgroups + TMA warp
-  static constexpr int SMEM = (QT + 2 * KS) * TILE_BYTES + 1024 + 256;
+struct AttnCfg {
+  static constexpr int NWG = 2;                                    // consumer warpgroups
+  static constexpr int KS = 3;                                     // K / V ring depth
+  static constexpr int THREADS = 128 * (NWG + 1);                  // consumer warpgroups + producer warpgroup
+  static constexpr int SMEM = NWG * QTILE_BYTES + 2 * KS * TILE_BYTES + 1024 + 256;
+  // Register split after setmaxnreg.  The warpgroups can only redistribute what the CTA was given at launch (the
+  // __launch_bounds__ cap, 168 x 384 threads): an increase the CTA cannot cover would wait forever.
+  static constexpr int LAUNCH_REGS = (65536 / THREADS) / 8 * 8;
+  static constexpr int PRODUCER_REGS = 24;
+  static constexpr int CONSUMER_REGS = 240;
+  static_assert(128 * PRODUCER_REGS + 128 * NWG * CONSUMER_REGS <= LAUNCH_REGS * THREADS, "register split exceeds the launch allocation");
 };
 constexpr int OSTR = HD + 1;                 // fp32 row stride of the O tile staged for the epilogue (conflict-free reads)
 // the staged O tiles + (m, l) rows overlay the Q and K stages
-static_assert(AT_BM * OSTR * 4 + AT_BM * 8 <= (1 + AttnCfg<1>::KS) * TILE_BYTES, "O staging must fit over the Q / K stages");
-static_assert(2 * (AT_BM * OSTR * 4 + AT_BM * 8) <= (2 + AttnCfg<2>::KS) * TILE_BYTES, "O staging must fit over the Q / K stages");
+static_assert(AttnCfg::NWG * (AT_BM * OSTR * 4 + AT_BM * 8) <= AttnCfg::NWG * QTILE_BYTES + AttnCfg::KS * TILE_BYTES,
+              "O staging must fit over the Q / K stages");
 
 struct AttnParams {
   int Nq, Nk0, Nk1;
@@ -52,7 +69,7 @@ struct AttnParams {
   long long ldo;
   float* part_o;             // [splits, B*Nq, H*64] fp32 unnormalised  (splits > 1)
   float* part_ml;            // [splits, B*Nq, H, 2]  (m_used * sl2, l)
-  int* split_cnt;            // [B, H, ceil(Nq/128)] arrival counters (zero on entry, reset by the last arriver)
+  int* split_cnt;            // [B, H, ceil(Nq/64)] arrival counters (zero on entry, reset by the last arriver)
   int H;
   long long rows_total;      // B * Nq
   unsigned long long* trace; // debug only (m3r_debug_trace): per-CTA clock stamps, 64 words per CTA; normally null
@@ -122,23 +139,86 @@ template <bool BF16> __device__ __forceinline__ uint32_t packp(float lo, float h
   return r;
 }
 
-template <bool BF16, int QT, int CS>
-__global__ void __launch_bounds__(AttnCfg<QT>::THREADS, QT == 1 ? 2 : 1)
+
+// Online softmax of one 128-key score tile, in place: s <- 2^(s * sl2 - m_used * sl2), with masking, the lazy max
+// refresh and the row sums.  alpha = the factor O must be rescaled by before P V of this tile is added.
+__device__ __forceinline__ void softmax_tile(float (&s)[64], const TileIt& it, int lo, int hi, int fc, float sl2,
+                                             float (&m_used)[2], float (&l_run)[2], float (&alpha)[2]) {
+  if (it.mask) {
+#pragma unroll
+    for (int i = 0; i < 64; ++i) {
+      const int lc = (i >> 2) * 8 + fc + (i & 1);
+      const int g = it.g0 + lc;
+      if (!(lc < it.nvalid && !(g >= lo && g < hi))) s[i] = -INFINITY;
+    }
+  }
+#pragma unroll
+  for (int rr = 0; rr < 2; ++rr) {
+    float mx = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < 32; ++i) mx = fmaxf(mx, s[(i >> 1) * 4 + rr * 2 + (i & 1)]);
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+    // lazy rescaling: refresh the folded max only when it is stale by more than 2^8
+    alpha[rr] = 1.f;
+    if (mx > -INFINITY && (m_used[rr] == -INFINITY || (mx - m_used[rr]) * sl2 > RESCALE_THRESHOLD)) {
+      alpha[rr] = (m_used[rr] == -INFINITY) ? 0.f : ex2((m_used[rr] - mx) * sl2);
+      m_used[rr] = mx;
+    }
+    l_run[rr] *= alpha[rr];
+  }
+  const float moff0 = (m_used[0] == -INFINITY) ? 0.f : m_used[0] * sl2;
+  const float moff1 = (m_used[1] == -INFINITY) ? 0.f : m_used[1] * sl2;
+#pragma unroll
+  for (int nb = 0; nb < 16; ++nb) {
+    s[nb * 4] = ex2(fmaf(s[nb * 4], sl2, -moff0)); s[nb * 4 + 1] = ex2(fmaf(s[nb * 4 + 1], sl2, -moff0));
+    s[nb * 4 + 2] = ex2(fmaf(s[nb * 4 + 2], sl2, -moff1)); s[nb * 4 + 3] = ex2(fmaf(s[nb * 4 + 3], sl2, -moff1));
+    l_run[0] += s[nb * 4] + s[nb * 4 + 1];
+    l_run[1] += s[nb * 4 + 2] + s[nb * 4 + 3];
+  }
+}
+
+// P in the A-operand fragment order: k-step kk covers keys 16 kk .. 16 kk + 15 = score blocks 2 kk, 2 kk + 1
+// pa[4 kk ..] = {rows fr: keys 16kk + fc.., rows fr+8: same, rows fr: keys 16kk + 8 + fc.., rows fr+8: same}
+template <bool BF16> __device__ __forceinline__ void pack_p(const float (&s)[64], uint32_t (&pa)[32]) {
+#pragma unroll
+  for (int nb = 0; nb < 16; ++nb) {
+    pa[(nb >> 1) * 4 + (nb & 1) * 2] = packp<BF16>(s[nb * 4], s[nb * 4 + 1]);
+    pa[(nb >> 1) * 4 + (nb & 1) * 2 + 1] = packp<BF16>(s[nb * 4 + 2], s[nb * 4 + 3]);
+  }
+}
+
+// S[64 x 128] = Q K^T over the 4 k16 steps of head_dim 64 (16 head dims: +32 B inside the swizzle atom)
+template <bool BF16> __device__ __forceinline__ void issue_qk(float (&s)[64], uint64_t qdesc, uint64_t kdesc) {
+#pragma unroll
+  for (int k = 0; k < HD / 16; ++k) Wgmma<128, BF16>::ss(s, qdesc + 2 * k, kdesc + 2 * k, k ? 1 : 0);
+}
+
+// O[64 x 64] += P[64 x 128] V[128 x 64] over 8 k16 steps (16 V rows: +2048 B)
+template <bool BF16> __device__ __forceinline__ void issue_pv(float (&o)[32], const uint32_t (&pa)[32], uint64_t vdesc) {
+#pragma unroll
+  for (int kk = 0; kk < AT_BN / 16; ++kk) {
+    const uint32_t a[4] = {pa[kk * 4], pa[kk * 4 + 1], pa[kk * 4 + 2], pa[kk * 4 + 3]};
+    WgmmaRS<BF16>::n64_tb(o, a, vdesc + (uint64_t)((kk * 16 * 128) >> 4));
+  }
+}
+
+template <bool BF16>
+__global__ void __launch_bounds__(AttnCfg::THREADS, 1)
 attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK0,
             const __grid_constant__ CUtensorMap tmV0, const __grid_constant__ CUtensorMap tmK1,
             const __grid_constant__ CUtensorMap tmV1, const AttnParams p) {
-  using Cfg = AttnCfg<QT>;
+  using Cfg = AttnCfg;
+  constexpr int NWG = Cfg::NWG;
   constexpr int KS = Cfg::KS;
-  constexpr int NWG = 2 * QT;                                   // consumer warpgroups (64 query rows each)
   constexpr int CT = 128 * NWG;                                 // consumer threads
   constexpr int TMA_WARP = 4 * NWG;
-  constexpr int SW = AT_BN / CS;                                // score columns per softmax pass
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem;                                   // QT tiles
-  uint8_t* sK = smem + QT * TILE_BYTES;                 // KS tiles
-  uint8_t* sV = smem + (QT + KS) * TILE_BYTES;          // KS tiles
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (QT + 2 * KS) * TILE_BYTES);
+  uint8_t* sQ = smem;                                   // NWG x 64 rows
+  uint8_t* sK = smem + NWG * QTILE_BYTES;               // KS tiles
+  uint8_t* sV = sK + KS * TILE_BYTES;                   // KS tiles
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + KS * TILE_BYTES);
   uint64_t* q_full = bars;             // [1]
   uint64_t* k_full = bars + 1;         // [KS]
   uint64_t* k_empty = k_full + KS;     // [KS]
@@ -147,12 +227,13 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
 
   M3R_TR(const unsigned long long t_entry = p.trace ? gtime_ns() : 0ull;)
   const int warp = threadIdx.x >> 5;
-  const int qblk = blockIdx.x, h = blockIdx.y;
+  const int wg = threadIdx.x >> 7;
+  const int h = blockIdx.y;
   const int b = blockIdx.z / p.splits, split = blockIdx.z % p.splits;
   const int kvb = b / p.kv_group;
   const int lo = p.skip_len > 0 ? p.skip_lo + (b % p.kv_group) * p.skip_step : 0;
   const int hi = p.skip_len > 0 ? lo + p.skip_len : 0;
-  const int q0 = qblk * QT * AT_BM;
+  const int q0 = blockIdx.x * NWG * AT_BM;
 
   // this CTA's share [i0, i1) of the enumerated key tiles
   const TileMap tiles(p.Nk0, p.Nk1, lo, hi);
@@ -173,11 +254,12 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
   griddep_wait();
   griddep_launch();
 
-  if (warp == TMA_WARP) {
-    // ------------------------------------------------------------------ TMA producer
-    if (elect_one() && n_tiles > 0) {
-      mbar_arrive_expect_tx(q_full, QT * TILE_BYTES);
-      for (int x = 0; x < QT; ++x) tma_load_3d(sQ + x * TILE_BYTES, &tmQ, q_full, h * HD, q0 + x * AT_BM, b);
+  if (wg == NWG) {
+    // ------------------------------------------------------------------ TMA producer warpgroup
+    setmaxnreg_dec<Cfg::PRODUCER_REGS>();
+    if (warp == TMA_WARP && elect_one() && n_tiles > 0) {
+      mbar_arrive_expect_tx(q_full, NWG * QTILE_BYTES);
+      for (int x = 0; x < NWG; ++x) tma_load_3d(sQ + x * QTILE_BYTES, &tmQ, q_full, h * HD, q0 + x * AT_BM, b);
       for (int j = 0; j < n_tiles; ++j) {
         const TileIt it = tiles.get(i0 + j);
         const int st = j % KS;
@@ -194,13 +276,13 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
     }
     return;
   }
+  setmaxnreg_inc<Cfg::CONSUMER_REGS>();
 
   // ------------------------------------------------------------------ consumer warpgroup: 64 query rows
-  const int wg = warp >> 2;
-  const int x = wg >> 1;                       // query tile
   const int wl = warp & 3, lane = threadIdx.x & 31;
-  const int fr = (wg & 1) * 64 + wl * 16 + (lane >> 2);     // fragment rows fr and fr + 8 of the query tile
+  const int fr = wl * 16 + (lane >> 2);                     // fragment rows fr and fr + 8 of the warpgroup's 64 rows
   const int fc = 2 * (lane & 3);                            // fragment column offset inside every 8-column block
+  const bool leader = wl == 0 && lane == 0;                 // arrives on the ring's empty barriers for the warpgroup
   float o[32];                                 // O[64 x 64] fragment
 #pragma unroll
   for (int i = 0; i < 32; ++i) o[i] = 0.f;
@@ -211,81 +293,52 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
            tr = p.trace + 128ull * ((blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x);
          if (tr) { tr[0] = t_entry; tr[1] = gtime_ns(); tr[2] = smid(); tr[3] = (unsigned long long)n_tiles; })
   if (n_tiles > 0) {
-    const uint64_t qdesc = smem_desc_sw128(smem_u32(sQ + x * TILE_BYTES + (wg & 1) * 64 * 128));
+    const uint64_t qdesc = smem_desc_sw128(smem_u32(sQ + wg * QTILE_BYTES));
+    float s[64];                               // S / P of the tile in flight (fp32)
+    uint32_t pa[32];                           // P of the previous tile, packed: the A operand of its P V
+    float alpha[2];
     mbar_wait(q_full, 0);
-    for (int j = 0; j < n_tiles; ++j) {
-      const TileIt it = tiles.get(i0 + j);
-      const int st = j % KS;
-      const uint32_t ph = (j / KS) & 1;
-      mbar_wait(&k_full[st], ph);
+    // tile 0: scores and softmax only
+    mbar_wait(&k_full[0], 0);
+    wgmma_fence();
+    issue_qk<BF16>(s, qdesc, smem_desc_sw128(smem_u32(sK)));
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+    if (leader) mbar_arrive(&k_empty[0]);
+    softmax_tile(s, tiles.get(i0), lo, hi, fc, p.sl2, m_used, l_run, alpha);
+    pack_p<BF16>(s, pa);
+    for (int j = 1; j < n_tiles; ++j) {
+      const int st = j % KS, pst = (j - 1) % KS;
       M3R_TR(if (tr && j < 12) tr[8 + 4 * j] = gtime_ns();)
-      const uint64_t kdesc = smem_desc_sw128(smem_u32(sK + st * TILE_BYTES));
-      const uint64_t vdesc = smem_desc_sw128(smem_u32(sV + st * TILE_BYTES));
-      // the 128-key tile in CS column slices of SW keys: S[64 x SW] = Q K_slice^T, online softmax, O += P V_slice
-#pragma unroll 1
-      for (int hh = 0; hh < CS; ++hh) {
-        float s[SW / 2];
-        wgmma_fence();
+      mbar_wait(&k_full[st], (j / KS) & 1);
+      mbar_wait(&v_full[pst], ((j - 1) / KS) & 1);
+      wgmma_fence();
+      issue_qk<BF16>(s, qdesc, smem_desc_sw128(smem_u32(sK + st * TILE_BYTES)));
+      wgmma_commit();
+      issue_pv<BF16>(o, pa, smem_desc_sw128(smem_u32(sV + pst * TILE_BYTES)));
+      wgmma_commit();
+      wgmma_wait<1>();                          // the scores of tile j are in; P V of tile j - 1 may still run
+      reg_fence(s);
+      if (leader) mbar_arrive(&k_empty[st]);
+      softmax_tile(s, tiles.get(i0 + j), lo, hi, fc, p.sl2, m_used, l_run, alpha);
+      wgmma_wait<0>();
+      reg_fence(o);
+      reg_fence(pa);
+      if (leader) mbar_arrive(&v_empty[pst]);
 #pragma unroll
-        for (int k = 0; k < HD / 16; ++k)        // K rows SW hh.. : +SW * 128 B; 16 head dims: +32 B
-          Wgmma<SW, BF16>::ss(s, qdesc + 2 * k, kdesc + (uint64_t)(hh * SW * 8) + 2 * k, k ? 1 : 0);
-        wgmma_commit();
-        wgmma_wait<0>();
-        reg_fence(s);
-        if (hh == CS - 1 && wl == 0 && lane == 0) mbar_arrive(&k_empty[st]);      // this warpgroup's last read of the K tile
-        if (it.mask) {
-#pragma unroll
-          for (int i = 0; i < SW / 2; ++i) {
-            const int lc = hh * SW + (i >> 2) * 8 + fc + (i & 1);
-            const int g = it.g0 + lc;
-            if (!(lc < it.nvalid && !(g >= lo && g < hi))) s[i] = -INFINITY;
-          }
-        }
-        float alpha[2];
-#pragma unroll
-        for (int rr = 0; rr < 2; ++rr) {
-          float mx = -INFINITY;
-#pragma unroll
-          for (int i = 0; i < SW / 4; ++i) mx = fmaxf(mx, s[(i >> 1) * 4 + rr * 2 + (i & 1)]);
-          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-          // lazy rescaling: refresh the folded max only when it is stale by more than 2^8
-          alpha[rr] = 1.f;
-          if (mx > -INFINITY && (m_used[rr] == -INFINITY || (mx - m_used[rr]) * p.sl2 > RESCALE_THRESHOLD)) {
-            alpha[rr] = (m_used[rr] == -INFINITY) ? 0.f : ex2((m_used[rr] - mx) * p.sl2);
-            m_used[rr] = mx;
-          }
-          l_run[rr] *= alpha[rr];
-        }
-#pragma unroll
-        for (int i = 0; i < 32; ++i) o[i] *= alpha[(i >> 1) & 1];
-        const float moff0 = (m_used[0] == -INFINITY) ? 0.f : m_used[0] * p.sl2;
-        const float moff1 = (m_used[1] == -INFINITY) ? 0.f : m_used[1] * p.sl2;
-        // P in the A-operand fragment order: k-step kk covers keys 16 kk .. 16 kk + 15 = score blocks 2 kk, 2 kk + 1
-        uint32_t pa[SW / 16][4];
-#pragma unroll
-        for (int nb = 0; nb < SW / 8; ++nb) {
-          const float a0 = ex2(fmaf(s[nb * 4], p.sl2, -moff0)), a1 = ex2(fmaf(s[nb * 4 + 1], p.sl2, -moff0));
-          const float a2 = ex2(fmaf(s[nb * 4 + 2], p.sl2, -moff1)), a3 = ex2(fmaf(s[nb * 4 + 3], p.sl2, -moff1));
-          l_run[0] += a0 + a1;
-          l_run[1] += a2 + a3;
-          pa[nb >> 1][(nb & 1) * 2] = packp<BF16>(a0, a1);
-          pa[nb >> 1][(nb & 1) * 2 + 1] = packp<BF16>(a2, a3);
-        }
-        if (hh == 0) mbar_wait(&v_full[st], ph);
-        wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < SW / 16; ++kk) {
-          // A = {rows fr: keys 16kk + fc.., rows fr+8: same, rows fr: keys 16kk + 8 + fc.., rows fr+8: same}
-          const uint32_t a[4] = {pa[kk][0], pa[kk][1], pa[kk][2], pa[kk][3]};
-          WgmmaRS<BF16>::n64_tb(o, a, vdesc + (uint64_t)((hh * SW + kk * 16) * 128 >> 4));
-        }
-        wgmma_commit();
-        wgmma_wait<0>();
-        reg_fence(o);
-        if (hh == CS - 1 && wl == 0 && lane == 0) mbar_arrive(&v_empty[st]);
-      }
+      for (int i = 0; i < 32; ++i) o[i] *= alpha[(i >> 1) & 1];
+      pack_p<BF16>(s, pa);
     }
+    const int lst = (n_tiles - 1) % KS;
+    mbar_wait(&v_full[lst], ((n_tiles - 1) / KS) & 1);
+    wgmma_fence();
+    issue_pv<BF16>(o, pa, smem_desc_sw128(smem_u32(sV + lst * TILE_BYTES)));
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(o);
+    reg_fence(pa);
+    if (leader) mbar_arrive(&v_empty[lst]);
   }
   M3R_TR(if (tr) tr[4] = gtime_ns();)
 #pragma unroll
@@ -298,27 +351,27 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
   // takes one row and 32 of its 64 columns: the layout of the stores, the split partials and the merge below.
   asm volatile("bar.sync 1, %0;" ::"n"(CT) : "memory");
   {
-    float* so = reinterpret_cast<float*>(smem) + x * (AT_BM * OSTR);
+    float* so = reinterpret_cast<float*>(smem) + wg * (AT_BM * OSTR);
 #pragma unroll
     for (int nb = 0; nb < 8; ++nb) {
       so[fr * OSTR + nb * 8 + fc] = o[nb * 4]; so[fr * OSTR + nb * 8 + fc + 1] = o[nb * 4 + 1];
       so[(fr + 8) * OSTR + nb * 8 + fc] = o[nb * 4 + 2]; so[(fr + 8) * OSTR + nb * 8 + fc + 1] = o[nb * 4 + 3];
     }
-    float2* sml = reinterpret_cast<float2*>(reinterpret_cast<float*>(smem) + QT * AT_BM * OSTR) + x * AT_BM;
+    float2* sml = reinterpret_cast<float2*>(reinterpret_cast<float*>(smem) + NWG * AT_BM * OSTR) + wg * AT_BM;
     if ((lane & 3) == 0) { sml[fr] = make_float2(m_used[0], l_run[0]); sml[fr + 8] = make_float2(m_used[1], l_run[1]); }
   }
   asm volatile("bar.sync 1, %0;" ::"n"(CT) : "memory");
-  const int row = threadIdx.x & 127;
-  const int half = (threadIdx.x >> 7) & 1;
-  const int q_idx = q0 + x * AT_BM + row;
+  const int row = threadIdx.x & (AT_BM - 1);
+  const int half = (threadIdx.x >> 6) & 1;
+  const int q_idx = q0 + wg * AT_BM + row;
   constexpr int OC = HD / 2;
   float acc[OC];
   float m_row, l_row;
   {
-    const float* so = reinterpret_cast<const float*>(smem) + x * (AT_BM * OSTR) + row * OSTR + half * OC;
+    const float* so = reinterpret_cast<const float*>(smem) + wg * (AT_BM * OSTR) + row * OSTR + half * OC;
 #pragma unroll
     for (int d = 0; d < OC; ++d) acc[d] = so[d];
-    const float2 ml = (reinterpret_cast<const float2*>(reinterpret_cast<const float*>(smem) + QT * AT_BM * OSTR) + x * AT_BM)[row];
+    const float2 ml = (reinterpret_cast<const float2*>(reinterpret_cast<const float*>(smem) + NWG * AT_BM * OSTR) + wg * AT_BM)[row];
     m_row = ml.x; l_row = ml.y;
   }
   if (q_idx < p.Nq && p.splits == 1 && p.exp_o != nullptr) {
@@ -341,15 +394,15 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
       o4[t] = w;
     }
   }
-  // key-range splits: unnormalised partial (O, m, l) of this CTA.  Layout [split][unit = (b, h, query tile)][16 column
-  // chunks][128 rows] float4 (and [split][unit][128 rows] float2): lanes are consecutive rows, so both these stores and
-  // the merge's loads are fully coalesced 512 B requests.
+  // key-range splits: unnormalised partial (O, m, l) of this CTA.  Layout [split][unit = (b, h, 64-row query tile)]
+  // [16 column chunks][64 rows] float4 (and [split][unit][64 rows] float2): lanes are consecutive rows, so both these
+  // stores and the merge's loads are fully coalesced 512 B requests.
   constexpr int CH = 8;                   // float4 column chunks per thread
   const int n_qtiles = (p.Nq + AT_BM - 1) / AT_BM;
-  const long long unit = ((long long)b * p.H + h) * n_qtiles + (q0 / AT_BM + x);
+  const long long unit = ((long long)b * p.H + h) * n_qtiles + (q0 / AT_BM + wg);
   const long long n_units = (long long)gridDim.z / p.splits * p.H * n_qtiles;
-  // (a second query tile entirely past Nq has no unit of its own: it takes no part in the split bookkeeping)
-  if (p.splits > 1 && q0 + x * AT_BM < p.Nq) {
+  // (a warpgroup whose rows are all past Nq has no unit of its own: it takes no part in the split bookkeeping)
+  if (p.splits > 1 && q0 + wg * AT_BM < p.Nq) {
     float4* o4 = reinterpret_cast<float4*>(p.part_o) + ((long long)split * n_units + unit) * (16 * AT_BM) + (half * CH) * AT_BM + row;
 #pragma unroll
     for (int t = 0; t < CH; ++t) o4[t * AT_BM] = make_float4(acc[4 * t], acc[4 * t + 1], acc[4 * t + 2], acc[4 * t + 3]);
@@ -358,20 +411,21 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
           make_float2(m_row == -INFINITY ? -INFINITY : m_row * p.sl2, l_row);
   }
   M3R_TR(if (tr) tr[5] = gtime_ns();)
-  if (p.splits > 1 && q0 + x * AT_BM < p.Nq) {
+  if (p.splits > 1 && q0 + wg * AT_BM < p.Nq) {
     // ---- merge of the key-range splits by the last CTA to finish this (batch, head, query tile):
     // out = sum_s O_s 2^(m_s - m) / sum_s l_s 2^(m_s - m).  No extra kernel launch on the one-view-per-step chain.
-    __shared__ int s_last[2];
+    // Named barriers 2 .. 2 + NWG - 1: one per warpgroup (barrier 1 is the consumers' O staging above).
+    __shared__ int s_last[NWG];
     __threadfence();                                              // partials visible device-wide
-    asm volatile("bar.sync %0, 256;" ::"r"(2 + x) : "memory");    // the softmax threads of this query tile
+    asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
     int* cnt = p.split_cnt + unit;
-    if (row == 0 && half == 0) {
+    if ((threadIdx.x & 127) == 0) {
       const int prev = atomicAdd(cnt, 1);
-      s_last[x] = (prev == p.splits - 1);
+      s_last[wg] = (prev == p.splits - 1);
       if (prev == p.splits - 1) *cnt = 0;                         // self-cleaning for the next launch
     }
-    asm volatile("bar.sync %0, 256;" ::"r"(2 + x) : "memory");
-    if (s_last[x]) {
+    asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+    if (s_last[wg]) {
       __threadfence();
       const float2* mlp = reinterpret_cast<const float2*>(p.part_ml) + unit * AT_BM + row;
       const float4* op = reinterpret_cast<const float4*>(p.part_o) + unit * (16 * AT_BM) + (half * CH) * AT_BM + row;
@@ -433,19 +487,35 @@ M3R_TR(if (p.trace && threadIdx.x == 0)
          p.trace[128ull * ((blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) + 6] = gtime_ns();)
 }
 
-template <bool BF16, int QT, int CS>
+// Sets the function attributes (per device: they are per context) and returns how many CTAs an SM holds, from the
+// kernel's actual registers and shared memory; checks that the launch allocation covers the register split.
+template <bool BF16> static int attn_resident_ctas() {
+  static int resident[64] = {};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return set_error("attention: bad current device"), -1;
+  if (resident[dev] == 0) {
+    using Cfg = AttnCfg;
+    cudaError_t e = cudaFuncSetAttribute(attn_kernel<BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
+    if (e != cudaSuccess) return set_error("attention: cudaFuncSetAttribute: %s", cudaGetErrorString(e)), -1;
+    cudaFuncAttributes fa;
+    e = cudaFuncGetAttributes(&fa, attn_kernel<BF16>);
+    if (e != cudaSuccess) return set_error("attention: cudaFuncGetAttributes: %s", cudaGetErrorString(e)), -1;
+    if (fa.numRegs < Cfg::LAUNCH_REGS)
+      return set_error("attention: kernel built with %d registers per thread, the register split needs %d", fa.numRegs, Cfg::LAUNCH_REGS), -1;
+    int n = 0;
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, attn_kernel<BF16>, Cfg::THREADS, Cfg::SMEM);
+    if (e != cudaSuccess || n < 1) return set_error("attention: occupancy query failed: %s", cudaGetErrorString(e)), -1;
+    resident[dev] = n;
+  }
+  return resident[dev];
+}
+
+template <bool BF16>
 static int launch_attn(const CUtensorMap& tmQ, const CUtensorMap& tmK0, const CUtensorMap& tmV0, const CUtensorMap& tmK1,
                        const CUtensorMap& tmV1, const AttnParams& p, int B, cudaStream_t s) {
-  using Cfg = AttnCfg<QT>;
-  static bool attr_set[64] = {};               // per device (function attributes are per context)
-  int dev = 0; cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && !attr_set[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(attn_kernel<BF16, QT, CS>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
-    if (e != cudaSuccess) return set_error("attention: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-    attr_set[dev] = true;
-  }
-  dim3 grid((p.Nq + QT * AT_BM - 1) / (QT * AT_BM), p.H, B * p.splits);
-  cudaError_t e = launch_pdl(attn_kernel<BF16, QT, CS>, grid, dim3(Cfg::THREADS), Cfg::SMEM, s, tmQ, tmK0, tmV0, tmK1, tmV1, p);
+  using Cfg = AttnCfg;
+  dim3 grid((p.Nq + Cfg::NWG * AT_BM - 1) / (Cfg::NWG * AT_BM), p.H, B * p.splits);
+  cudaError_t e = launch_pdl(attn_kernel<BF16>, grid, dim3(Cfg::THREADS), Cfg::SMEM, s, tmQ, tmK0, tmV0, tmK1, tmV1, p);
   if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) return set_error("attention launch: %s", cudaGetErrorString(e));
   count_launch();
@@ -477,55 +547,43 @@ extern "C" int m3r_attention(const m3r_attn_args* a, void* stream) {
   cudaStream_t cs = reinterpret_cast<cudaStream_t>(stream);
   const int Bkv = a->B / a->kv_group;
   CUtensorMap tmQ, tmK0, tmV0, tmK1, tmV1;
-  auto mk3 = [&](CUtensorMap* m, const void* base, int64_t ld, int64_t rows, int64_t bstride_rows, int64_t nb) {
+  auto mk3 = [&](CUtensorMap* m, const void* base, int64_t ld, int64_t rows, int64_t bstride_rows, int64_t nb, uint32_t box_rows) {
     return make_tmap_3d(m, base, a->is_bf16, (uint64_t)a->H * HD, (uint64_t)rows, (uint64_t)nb, (uint64_t)ld,
-                        (uint64_t)bstride_rows * (uint64_t)ld, HD, 128);
+                        (uint64_t)bstride_rows * (uint64_t)ld, HD, box_rows);
   };
-  if (mk3(&tmQ, a->Q, a->ldq, a->Nq, a->Nq, a->B)) return 1;
+  if (mk3(&tmQ, a->Q, a->ldq, a->Nq, a->Nq, a->B, AT_BM)) return 1;
   if (a->Nk0 > 0) {
-    if (mk3(&tmK0, a->K0, a->ldk0, a->Nk0, a->kv_bstride0, Bkv)) return 1;
-    if (mk3(&tmV0, a->V0, a->ldk0, a->Nk0, a->kv_bstride0, Bkv)) return 1;
+    if (mk3(&tmK0, a->K0, a->ldk0, a->Nk0, a->kv_bstride0, Bkv, AT_BN)) return 1;
+    if (mk3(&tmV0, a->V0, a->ldk0, a->Nk0, a->kv_bstride0, Bkv, AT_BN)) return 1;
   } else { tmK0 = tmQ; tmV0 = tmQ; }
   if (a->Nk1 > 0) {
-    if (mk3(&tmK1, a->K1, a->ldk1, a->Nk1, a->kv_bstride1, Bkv)) return 1;
-    if (mk3(&tmV1, a->V1, a->ldk1, a->Nk1, a->kv_bstride1, Bkv)) return 1;
+    if (mk3(&tmK1, a->K1, a->ldk1, a->Nk1, a->kv_bstride1, Bkv, AT_BN)) return 1;
+    if (mk3(&tmV1, a->V1, a->ldk1, a->Nk1, a->kv_bstride1, Bkv, AT_BN)) return 1;
   } else { tmK1 = tmK0; tmV1 = tmV0; }
 
-  // ---- shape heuristics (tools/prof_attn.py `sweep` / `longmem` compares the variants on a given GPU):
-  //  * enough work for ~half a wave of 2-tile CTAs -> QT=2 (K/V tiles shared by two query tiles), no split;
-  //  * otherwise (one view per step) QT=1, two CTAs per SM, and the key range split so that ~2 CTAs per SM exist,
-  //    keeping at least 4 key tiles per split; the last CTA of a (batch, head, tile) to finish merges the partials.
+  // ---- key splits, from a cost model in units of one CTA's pass over one key tile (CTAs of 128 query rows, one per
+  // SM).  CTAs run in waves of (resident CTAs per SM x SMs); each CTA pays about 4 tile passes of prologue (Q load,
+  // pipeline fill) and epilogue; a split launch pays the partial stores plus the merge, which reads every split's
+  // partial.  Both constants were fitted to tools/prof_attn.py `sweep` / `longmem` on H100 SXM (132 SMs), where this
+  // picks the measured best split count or one within 5 % of it.  M3R_ATTN_SPLITS forces a split count.
   const int sms = num_sms();
   const int key_tiles = (a->Nk0 + AT_BN - 1) / AT_BN + (a->Nk1 + AT_BN - 1) / AT_BN;   // upper bound
-  const int ctas2 = ((a->Nq + 255) / 256) * a->H * a->B;
-  const int ctas1 = ((a->Nq + 127) / 128) * a->H * a->B;
-  int qt = (a->Nq > 128 && 2 * ctas2 >= sms) ? 2 : 1;
-  //  * one view against a LONG memory (>= ~64 views): two query tiles per CTA halve the K/V bytes each SM pulls per flop,
-  //    which is what bounds the QT=1 form there; the key range is split to fill the SMs (below ~50 views QT=1 with
-  //    splits stays ahead)
-  const bool long_keys = qt == 1 && a->Nq > 128 && key_tiles >= 384 && ctas2 < sms;
-  if (long_keys) qt = 2;
-  if (const char* f = getenv("M3R_ATTN_QT")) { const int v = atoi(f); if (v == 1 || v == 2) qt = v; }
+  const bool split_ok = (long long)a->B * a->H * ((a->Nq + AT_BM - 1) / AT_BM) <= 16384;   // counter table of the split path
+  const int resident = a->is_bf16 ? attn_resident_ctas<true>() : attn_resident_ctas<false>();
+  if (resident < 0) return 1;
   int splits = 1;
-  if (qt == 1 && ctas1 < 2 * sms) {
-    splits = (2 * sms + ctas1 / 2) / ctas1;
-    if (splits > key_tiles / 4) splits = key_tiles / 4;        // a split pays a partial store + merge: >= 4 tiles each
-  } else if (qt == 2 && long_keys) {
-    splits = (sms + ctas2 / 2) / ctas2;
-  } else if (qt == 2 && key_tiles >= 64) {
-    //  * throughput shapes whose CTA count is an awkward multiple of the SM count (13 views on one of 8 GPUs: 468 CTAs =
-    //    3.16 waves, 21 % of the last wave's SMs idle): split the long key range 2..4 ways when that fills the waves better
-    //    (every split keeps >= 16 key tiles, so the partial store + merge stays below a few percent)
-    auto eff = [&](int sp) { const long long c = (long long)ctas2 * sp; return (double)c / (double)(((c + sms - 1) / sms) * sms); };
-    double best = eff(1);
-    for (int sp = 2; sp <= 4 && key_tiles / sp >= 16; ++sp)
-      if (eff(sp) > best + 0.04) { best = eff(sp); splits = sp; }
+  if (const char* f = getenv("M3R_ATTN_SPLITS")) { const int v = atoi(f); if (v >= 1) splits = min(v, min(32, key_tiles)); }
+  else if (split_ok) {
+    const long long ctas = (long long)((a->Nq + AttnCfg::NWG * AT_BM - 1) / (AttnCfg::NWG * AT_BM)) * a->H * a->B;
+    const long long slots = (long long)resident * sms;
+    double best = 0.0;
+    for (int sp = 1; sp <= 32 && sp <= key_tiles; ++sp) {
+      const int chunk = (key_tiles + sp - 1) / sp;
+      const long long waves = (ctas * sp + slots - 1) / slots;
+      const double cost = waves * (chunk + 4.0) + (sp > 1 ? 4.0 + sp / 4.0 : 0.0);
+      if (sp == 1 || cost < best) { best = cost; splits = sp; }
+    }
   }
-  if (const char* f = getenv("M3R_ATTN_SPLITS")) { const int v = atoi(f); if (v >= 1) splits = v; }
-  if (splits > key_tiles) splits = key_tiles;
-  if (splits > 32) splits = 32;
-  if (splits < 1) splits = 1;
-  if ((long long)a->B * a->H * ((a->Nq + AT_BM - 1) / AT_BM) > 16384 && !getenv("M3R_ATTN_SPLITS")) splits = 1;   // counter table of the split path
   { const int chunk = (key_tiles + splits - 1) / splits; splits = (key_tiles + chunk - 1) / chunk; }   // no empty splits
 
   AttnParams p;
@@ -561,18 +619,11 @@ extern "C" int m3r_attention(const m3r_attn_args* a, void* stream) {
   }
   {
     const double nk_eff = (double)(a->Nk0 + a->Nk1 - a->skip_len);
-    ProfScope prof(qt == 2 ? PROF_ATTN_QT2 : PROF_ATTN_QT1, 4.0 * a->B * (double)a->H * a->Nq * nk_eff * HD,
+    // profiling categories: launches over the whole key range, and launches with key splits + in-kernel merge
+    ProfScope prof(splits == 1 ? PROF_ATTN_QT2 : PROF_ATTN_QT1, 4.0 * a->B * (double)a->H * a->Nq * nk_eff * HD,
                    2.0 * ((double)a->B * a->Nq * a->H * HD * 2 + (double)Bkv * (a->Nk0 + a->Nk1) * a->H * HD * 2), cs);
-    // score-tile column slices per softmax pass: 2 (default) = two 64-key passes per 128-key tile, half the score
-    // registers; 1 = one 128-key pass (M3R_ATTN_CS=1), which spills at the register budget of two CTAs per SM
-    int colsplit = 2;
-    if (const char* e = getenv("M3R_ATTN_CS")) { if (atoi(e) == 1) colsplit = 1; }
-    int rc;
-#define M3R_LAUNCH_ATTN(BF, QTV) (colsplit == 1 ? launch_attn<BF, QTV, 1>(tmQ, tmK0, tmV0, tmK1, tmV1, p, a->B, cs) \
-                                                : launch_attn<BF, QTV, 2>(tmQ, tmK0, tmV0, tmK1, tmV1, p, a->B, cs))
-    if (a->is_bf16) rc = qt == 2 ? M3R_LAUNCH_ATTN(true, 2) : M3R_LAUNCH_ATTN(true, 1);
-    else rc = qt == 2 ? M3R_LAUNCH_ATTN(false, 2) : M3R_LAUNCH_ATTN(false, 1);
-#undef M3R_LAUNCH_ATTN
+    const int rc = a->is_bf16 ? launch_attn<true>(tmQ, tmK0, tmV0, tmK1, tmV1, p, a->B, cs)
+                              : launch_attn<false>(tmQ, tmK0, tmV0, tmK1, tmV1, p, a->B, cs);
     if (rc) return rc;
   }
   return 0;

@@ -13,6 +13,9 @@ int num_sms();                                  // SM count of the current devic
 void count_launch();                            // bumps the kernel-launch counter (m3r_launch_count)
 
 // Optional per-category device timing (m3r_prof_*): CUDA events recorded on the launch stream around each kernel.
+// The attention kernel has one CTA shape; its two categories keep their historical names (bench.py prints them as
+// "attn_kernel<QT=2>" and "attn_kernel<QT=1>+split-merge"): PROF_ATTN_QT2 = launches over the whole key range,
+// PROF_ATTN_QT1 = launches with key splits and the in-kernel merge (the one-view update steps).
 enum ProfCat { PROF_GEMM256 = 0, PROF_GEMM128 = 1, PROF_GEMM64 = 2, PROF_ATTN_QT2 = 3, PROF_ATTN_QT1 = 4, PROF_LN = 5, PROF_OTHER = 6, PROF_NCAT = 7 };
 struct ProfScope {
   int slot;

@@ -109,6 +109,16 @@ template <int N> __device__ __forceinline__ void reg_fence(float (&d)[N]) {
 #pragma unroll
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+// the same for register A operands: keeps them live (their registers unreused) until the wgmma reading them has completed
+template <int N> __device__ __forceinline__ void reg_fence(uint32_t (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+r"(d[i])::"memory");
+}
+
+// ------------------------------------------------------------------ register reallocation between warpgroups
+// Executed by every warp of a warpgroup: a producer warpgroup gives registers back, consumer warpgroups take them.
+template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // D[64 x N] (+)= A[64 x 16] * B[16 x N], fp32 accumulate, both operands K-major in shared memory (descriptors).
 // Accumulator fragment of thread t of the warpgroup (warp w = t / 32, lane l): d[4j + e] is row 16w + l/4 (+8 for

@@ -12,7 +12,7 @@ def ref_attn(q, k, v, mask=None):
     return torch.softmax(s, -1) @ v.float()
 
 def case(dtype, Nm, n, N, B=2, H=12, env=None, tag=""):
-    for k in ("M3R_ATTN_QT", "M3R_ATTN_SPLITS"): os.environ.pop(k, None)
+    os.environ.pop("M3R_ATTN_SPLITS", None)
     if env: os.environ.update(env)
     D = H * 64
     cap = Nm + 77
@@ -43,8 +43,7 @@ def case(dtype, Nm, n, N, B=2, H=12, env=None, tag=""):
 for dt in (torch.float16, torch.bfloat16):
     for rep in range(2):
         case(dt, 1536, 2, 768, tag=f"default rep{rep}")
-    for env in ({"M3R_ATTN_QT": "2", "M3R_ATTN_SPLITS": "1"}, {"M3R_ATTN_QT": "2", "M3R_ATTN_SPLITS": "2"}, {"M3R_ATTN_QT": "2", "M3R_ATTN_SPLITS": "3"},
-                {"M3R_ATTN_QT": "1", "M3R_ATTN_SPLITS": "1"}, {"M3R_ATTN_QT": "1", "M3R_ATTN_SPLITS": "2"}):
+    for env in ({"M3R_ATTN_SPLITS": "1"}, {"M3R_ATTN_SPLITS": "2"}, {"M3R_ATTN_SPLITS": "3"}):
         case(dt, 1536, 2, 768, env=env, tag="forced")
     case(dt, 1536, 2, 768, B=1, tag="B=1")
     case(dt, 1536, 1, 768, tag="n=1")

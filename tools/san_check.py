@@ -10,9 +10,9 @@ ops.linear(a, w, torch.randn(512, device="cuda"), act="gelu")
 os.environ["M3R_GEMM_BN"] = "256"; ops.linear(a, w, None, out_dtype=torch.float32); os.environ.pop("M3R_GEMM_BN")
 q = torch.randn(2 * 300, 3 * 128, device="cuda").to(dt)
 ops.attention(q[:, :128], q[:, 128:256], q[:, 256:], B=2, H=2, Nq=300, Nk0=300)
-os.environ["M3R_ATTN_QT"] = "1"; os.environ["M3R_ATTN_SPLITS"] = "2"
+os.environ["M3R_ATTN_SPLITS"] = "2"
 ops.attention(q[:, :128], q[:, 128:256], q[:, 256:], B=2, H=2, Nq=300, Nk0=300)
-os.environ.pop("M3R_ATTN_QT"); os.environ.pop("M3R_ATTN_SPLITS")
+os.environ.pop("M3R_ATTN_SPLITS")
 enc = Dust3rEncoder(img_size=(64, 64), embed_dim=128, depth=1, num_heads=2).cuda()
 dec = MUSt3R(img_size=(64, 64), enc_embed_dim=128, embed_dim=128, depth=2, num_heads=2, feedback_type="single_mlp", memory_mode="kv", landscape_only=False).cuda()
 imgs, ts = syn.synthetic_views(3, 32, 48)

@@ -1,6 +1,6 @@
 """Timeline of the attention kernel from inside (m3r_debug_trace): where a launch's microseconds go.
 
-    python tools/trace_attn.py [Nk=7680] [B=1] [qt] [splits]
+    python tools/trace_attn.py [Nk=7680] [B=1] [splits]
 """
 import os, sys
 import torch
@@ -9,8 +9,7 @@ from must3r_b200 import ops, _lib  # noqa: E402
 
 Nk = int(sys.argv[1]) if len(sys.argv) > 1 else 7680
 B = int(sys.argv[2]) if len(sys.argv) > 2 else 1
-if len(sys.argv) > 3: os.environ["M3R_ATTN_QT"] = sys.argv[3]
-if len(sys.argv) > 4: os.environ["M3R_ATTN_SPLITS"] = sys.argv[4]
+if len(sys.argv) > 3: os.environ["M3R_ATTN_SPLITS"] = sys.argv[3]
 H, Nq, D = 12, 768, 768
 dt = torch.bfloat16
 q = torch.randn(B * Nq, D, device="cuda").to(dt)
