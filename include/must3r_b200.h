@@ -223,6 +223,31 @@ int m3r_postprocess(const float* pm, int64_t P, float* pts3d, float* pts3d_local
  * (must3r/slam/nns.py:57-62, called from must3r/slam/model.py:82). */
 int m3r_nn_min_dist(const float* queries, int32_t Q, const float* db, int64_t P, float* out, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------
+ * Input preprocessing of V RGB uint8 frames of one size: src [V, src_h, src_w, 3] uint8 (HWC; pixel stride 3 bytes,
+ * row pitch src_pitch bytes, frame stride src_vstride bytes - a crop view or a padded frame needs no copy) -> fp32
+ * [V, 3, h, w] images in the ImgNorm range (the encoder's input).  Two separable passes, horizontal then vertical;
+ * the host computes the coefficient tables (must3r_b200/engine/images.py): bounds [n, 2] int32 = (first source
+ * index, tap count <= k) and weights [n, k] per output column (x) / row (y).  `tmp` is device scratch.
+ * ------------------------------------------------------------------------------------------------- */
+/* Pillow's 8-bit Image.resize (LANCZOS / BICUBIC; dust3r/dust3r/utils/image.py:64-71 _resize_pil_image) bit for bit,
+ * then the crop box and ImgNorm of the SLAM front end (must3r/slam/model.py:99-120).  Weights are int32 with 22
+ * fractional bits.  The horizontal pass reads source rows [row0, row0 + rows) and writes tmp [V, rows, out_w, 3] uint8;
+ * y bounds are relative to row0.  Outputs (either may be NULL, not both): out_u8 [V, out_h, out_w, 3] = the resized
+ * image; out [V, 3, crop_h, crop_w] fp32 = ImgNorm of its box (crop_x, crop_y, crop_w, crop_h). */
+int m3r_resample_pil_u8(const uint8_t* src, int64_t src_pitch, int64_t src_vstride, int32_t V, int32_t src_h, int32_t src_w,
+                        const int32_t* xbounds, const int32_t* xweights, int32_t xk, int32_t out_w,
+                        const int32_t* ybounds, const int32_t* yweights, int32_t yk, int32_t out_h, int32_t row0,
+                        int32_t rows, uint8_t* tmp, uint8_t* out_u8, int32_t crop_x, int32_t crop_y, int32_t crop_w,
+                        int32_t crop_h, float* out, void* stream);
+/* Antialiased bilinear resize (aten _upsample_bilinear2d_aa, torchvision Resize) of ImgNorm(src) with fp32 weights:
+ * the demo's CenterCrop + Resize (must3r/tools/image.py:53-93, applied by must3r/demo/inference.py:63-76); src points at
+ * the crop's first pixel.  tmp: [V, 3, src_h, out_w] fp32; out: [V, 3, out_h, out_w] fp32. */
+int m3r_resize_aa_bilinear_u8(const uint8_t* src, int64_t src_pitch, int64_t src_vstride, int32_t V, int32_t src_h,
+                              int32_t src_w, const int32_t* xbounds, const float* xweights, int32_t xk, int32_t out_w,
+                              const int32_t* ybounds, const float* yweights, int32_t yk, int32_t out_h, float* tmp,
+                              float* out, void* stream);
+
 /* ===================================================================================================
  * Whole-model entry points: one call enqueues every kernel of a forward pass from C++ (no per-layer
  * Python/ctypes overhead).  Weight structs hold DEVICE pointers (16-bit matrices in nn.Linear layout,

@@ -84,6 +84,13 @@ SIGNATURES = {
     "m3r_unpatchify": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "m3r_postprocess": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "m3r_nn_min_dist": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
+    "m3r_resample_pil_u8": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32,
+                                      C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                      C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                      C.c_void_p, C.c_void_p]),
+    "m3r_resize_aa_bilinear_u8": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32,
+                                            C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
+                                            C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "m3r_peer_alloc": (C.c_int, [C.c_int64, C.POINTER(C.c_void_p)]),
     "m3r_peer_free": (C.c_int, [C.c_void_p]),
     "m3r_ipc_export": (C.c_int, [C.c_void_p, C.c_void_p]),

@@ -262,6 +262,49 @@ def unpatchify(proj: torch.Tensor, V: int, H: int, W: int, C_: int = 7) -> torch
     return out
 
 
+def _frames_u8(src: torch.Tensor):
+    """uint8 [V,H,W,3] CUDA view with pixel stride 3 and channel stride 1 (any row pitch / frame stride)."""
+    _req_cuda(src)
+    if src.dtype != torch.uint8 or src.dim() != 4 or src.shape[3] != 3 or src.stride(3) != 1 or src.stride(2) != 3:
+        raise ValueError(f"expected RGB uint8 frames [V,H,W,3] with interleaved channels, got {tuple(src.shape)} "
+                         f"{src.dtype} strides {src.stride()}")
+    return src.shape[0], src.shape[1], src.shape[2], src.stride(1), src.stride(0)
+
+
+def resample_pil_u8(src: torch.Tensor, tables, xk: int, yk: int, out_hw, row0: int, rows: int, tmp: torch.Tensor,
+                    crop, out: Optional[torch.Tensor] = None, out_u8: Optional[torch.Tensor] = None) -> None:
+    """Pillow-exact resize of uint8 frames src [V,H,W,3] to out_hw, then ImgNorm of the crop box (x, y, w, h) into `out`
+    [V,3,h,w] fp32 and/or the resized uint8 frames into `out_u8` [V,out_h,out_w,3].  tables: CUDA tensors whose first bytes
+    are (x bounds, x weights, y bounds, y weights), int32 (engine/images.py builds them); tmp: uint8 scratch of at least
+    V * rows * out_w * 3 bytes."""
+    V, H, W, pitch, vstride = _frames_u8(src)
+    _req_cuda(tmp, out, out_u8, *tables)
+    oh, ow = out_hw
+    assert tmp.numel() * tmp.element_size() >= V * rows * ow * 3
+    if out is not None:
+        assert out.dtype == torch.float32 and out.is_contiguous() and tuple(out.shape) == (V, 3, crop[3], crop[2])
+    if out_u8 is not None:
+        assert out_u8.dtype == torch.uint8 and out_u8.is_contiguous() and tuple(out_u8.shape) == (V, oh, ow, 3)
+    xb, xw, yb, yw = tables
+    _lib.check(_lib.lib().m3r_resample_pil_u8(_p(src), pitch, vstride, V, H, W, _p(xb), _p(xw), xk, ow, _p(yb), _p(yw), yk,
+                                              oh, row0, rows, _p(tmp), _p(out_u8), crop[0], crop[1], crop[2], crop[3],
+                                              _p(out), _stream()), "resample_pil_u8")
+
+
+def resize_aa_bilinear_u8(src: torch.Tensor, tables, xk: int, yk: int, out_hw, tmp: torch.Tensor, out: torch.Tensor) -> None:
+    """Antialiased bilinear resize (torchvision Resize) of ImgNorm(src), src uint8 [V,H,W,3] (a crop view is fine), into
+    out [V,3,out_h,out_w] fp32.  tables: (x bounds int32, x weights fp32, y bounds, y weights) CUDA tensors; tmp: scratch
+    of at least V * 3 * H * out_w fp32."""
+    V, H, W, pitch, vstride = _frames_u8(src)
+    _req_cuda(tmp, out, *tables)
+    oh, ow = out_hw
+    assert tmp.numel() * tmp.element_size() >= V * 3 * H * ow * 4
+    assert out.dtype == torch.float32 and out.is_contiguous() and tuple(out.shape) == (V, 3, oh, ow)
+    xb, xw, yb, yw = tables
+    _lib.check(_lib.lib().m3r_resize_aa_bilinear_u8(_p(src), pitch, vstride, V, H, W, _p(xb), _p(xw), xk, ow, _p(yb), _p(yw),
+                                                    yk, oh, _p(tmp), _p(out), _stream()), "resize_aa_bilinear_u8")
+
+
 def postprocess_raw(pm: torch.Tensor):
     _req_cuda(pm)
     assert pm.dtype == torch.float32 and pm.shape[-1] == 7

@@ -89,6 +89,26 @@ def synthetic_views(n_views: int, H: int, W: int, seed: int = 2) -> Tuple[torch.
     return imgs, true_shape
 
 
+def synthetic_frame(H: int, W: int, seed: int = 0) -> "np.ndarray":
+    """A camera-like RGB uint8 frame [H,W,3]: per-channel gradients plus noise, with hard-edged saturated blocks and a
+    black stripe, so that resampling filters ring against 0 and 255 and their clamping is exercised.  Integer arithmetic
+    only, so every machine regenerates the same bytes."""
+    g = torch.Generator(device="cpu").manual_seed(4000 + seed)
+    y = torch.arange(H, dtype=torch.int64)[:, None, None]
+    x = torch.arange(W, dtype=torch.int64)[None, :, None]
+    mix = torch.randint(0, 256, (1, 1, 3), generator=g)
+    img = (x * mix + y * (256 - mix)) * 120 // (256 * max(H + W - 2, 1))        # gradients, one direction per channel
+    img = img + ((3 * x + 2 * y + mix) % 48) * 2 + 40                              # a sawtooth texture
+    img = img + torch.randint(-40, 41, (H, W, 3), generator=g)                     # noise
+    for _ in range(6):                                                             # saturated rectangles, hard edges
+        y0, x0 = int(torch.randint(0, H, (1,), generator=g)), int(torch.randint(0, W, (1,), generator=g))
+        h = int(torch.randint(4, max(5, H // 4), (1,), generator=g))
+        w = int(torch.randint(4, max(5, W // 4), (1,), generator=g))
+        img[y0:y0 + h, x0:x0 + w] = 255 * torch.randint(0, 2, (3,), generator=g)
+    img[:, W // 3:W // 3 + max(1, W // 40)] = 0                                    # a black stripe next to bright content
+    return img.clamp(0, 255).to(torch.uint8).numpy()
+
+
 def rel_l2(a: torch.Tensor, b: torch.Tensor) -> float:
     """‖a−b‖₂ / ‖b‖₂ (b is the reference)."""
     a = a.detach().double().cpu()
