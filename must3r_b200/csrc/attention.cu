@@ -27,9 +27,6 @@
 // last CTA to finish a (batch, head, 64-row query tile) merges the partial (O, m, l) in-kernel.  The split
 // count comes from a wave-count cost model (m3r_attention).
 #include <math.h>
-#include <map>
-#include <mutex>
-#include <utility>
 #include "ptx.cuh"
 #include "m3r_internal.h"
 
@@ -487,27 +484,15 @@ M3R_TR(if (p.trace && threadIdx.x == 0)
          p.trace[128ull * ((blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) + 6] = gtime_ns();)
 }
 
-// Sets the function attributes (per device: they are per context) and returns how many CTAs an SM holds, from the
-// kernel's actual registers and shared memory; checks that the launch allocation covers the register split.
+// How many CTAs an SM holds, from the kernel's actual registers and shared memory (-1 after set_error); checks that the
+// launch allocation covers the register split.
 template <bool BF16> static int attn_resident_ctas() {
-  static int resident[64] = {};
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return set_error("attention: bad current device"), -1;
-  if (resident[dev] == 0) {
-    using Cfg = AttnCfg;
-    cudaError_t e = cudaFuncSetAttribute(attn_kernel<BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
-    if (e != cudaSuccess) return set_error("attention: cudaFuncSetAttribute: %s", cudaGetErrorString(e)), -1;
-    cudaFuncAttributes fa;
-    e = cudaFuncGetAttributes(&fa, attn_kernel<BF16>);
-    if (e != cudaSuccess) return set_error("attention: cudaFuncGetAttributes: %s", cudaGetErrorString(e)), -1;
-    if (fa.numRegs < Cfg::LAUNCH_REGS)
-      return set_error("attention: kernel built with %d registers per thread, the register split needs %d", fa.numRegs, Cfg::LAUNCH_REGS), -1;
-    int n = 0;
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, attn_kernel<BF16>, Cfg::THREADS, Cfg::SMEM);
-    if (e != cudaSuccess || n < 1) return set_error("attention: occupancy query failed: %s", cudaGetErrorString(e)), -1;
-    resident[dev] = n;
-  }
-  return resident[dev];
+  using Cfg = AttnCfg;
+  const KernelInfo k = kernel_setup((const void*)attn_kernel<BF16>, Cfg::SMEM, Cfg::THREADS);
+  if (k.resident == 0) return -1;
+  if (k.regs < Cfg::LAUNCH_REGS)
+    return set_error("attention: kernel built with %d registers per thread, the register split needs %d", k.regs, Cfg::LAUNCH_REGS), -1;
+  return k.resident;
 }
 
 template <bool BF16>
@@ -521,11 +506,6 @@ static int launch_attn(const CUtensorMap& tmQ, const CUtensorMap& tmK0, const CU
   count_launch();
   return 0;
 }
-
-// scratch for the split path, grown on demand (stream-ordered), one per (device, stream)
-struct SplitScratch { float* buf = nullptr; size_t cap = 0; };
-static std::mutex g_split_mu;
-static std::map<std::pair<int, cudaStream_t>, SplitScratch> g_split;      // per (device, stream): see gemm.cu emit_scratch
 
 }  // namespace m3r
 
@@ -601,20 +581,19 @@ extern "C" int m3r_attention(const m3r_attn_args* a, void* stream) {
     const size_t n_cnt = (size_t)a->B * a->H * ((a->Nq + AT_BM - 1) / AT_BM);
     if (n_cnt > CNT) return set_error("attention: too many (batch, head, tile) groups for the split path");
     const size_t need = CNT + (size_t)splits * n_cnt * AT_BM * (HD + 2);     // partial O + (m, l), padded to whole query tiles
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return set_error("attention: bad current device");
-    std::lock_guard<std::mutex> lock(g_split_mu);
-    SplitScratch& sc = g_split[std::make_pair(dev, cs)];
-    if (need > sc.cap) {
-      if (sc.buf) cudaFreeAsync(sc.buf, cs);
-      sc.buf = nullptr; sc.cap = 0;
+    RegistryLock lock;
+    StreamState* sc = stream_state(cs, lock);
+    if (!sc) return set_error("attention: no current device");
+    if (need > sc->split_cap) {
+      if (sc->split_buf) cudaFreeAsync(sc->split_buf, cs);
+      sc->split_buf = nullptr; sc->split_cap = 0;
       const size_t cap = need + need / 2;
-      if (cudaMallocAsync(&sc.buf, cap * sizeof(float), cs) != cudaSuccess) return set_error("attention: split scratch allocation failed");
-      if (cudaMemsetAsync(sc.buf, 0, CNT * sizeof(int), cs) != cudaSuccess) return set_error("attention: counter memset failed");
-      sc.cap = cap;
+      if (cudaMallocAsync(&sc->split_buf, cap * sizeof(float), cs) != cudaSuccess) return set_error("attention: split scratch allocation failed");
+      if (cudaMemsetAsync(sc->split_buf, 0, CNT * sizeof(int), cs) != cudaSuccess) return set_error("attention: counter memset failed");
+      sc->split_cap = cap;
     }
-    p.split_cnt = reinterpret_cast<int*>(sc.buf);
-    p.part_o = sc.buf + CNT;
+    p.split_cnt = reinterpret_cast<int*>(sc->split_buf);
+    p.part_o = sc->split_buf + CNT;
     p.part_ml = p.part_o + (size_t)splits * n_cnt * AT_BM * HD;
   }
   {

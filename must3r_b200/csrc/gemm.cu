@@ -6,9 +6,6 @@
 //   warp 8     : TMA producer (one elected lane) -- A and W tiles, 128B-swizzled, mbarrier ring
 // The producer keeps filling the ring for the next tile while the consumers drain the current one.  Tiles are walked
 // m-fastest so that co-resident CTAs share the weight tile in L2.
-#include <map>
-#include <mutex>
-#include <utility>
 #include "ptx.cuh"
 #include "m3r_internal.h"
 
@@ -514,34 +511,28 @@ static void fill_params(GemmParams& p, const m3r_gemm_args* a) {
 }
 
 // Scratch of the LayerNorm-emitting epilogue: partial row statistics + arrival / departure counters (+ split-K hand-over).
-// The CTAs of a launch spin on each other, so launches sharing a scratch must be ordered: the model code emits on the
-// caller's stream only, never on its side streams.
-struct EmitScratch { float2* stats = nullptr; unsigned int* sync = nullptr; float4* kpart = nullptr; unsigned int* kflag = nullptr; };
+// The CTAs of a launch spin on each other, so launches sharing a scratch must be ordered: there is one scratch per caller
+// stream (two host threads driving the model, as the reference's SLAM worker does, slam.py:533, must not share counters),
+// and the model code emits on the caller's stream only, never on its side streams.
 constexpr int EMIT_MAX_KSPLIT_TILES = 80;
 constexpr int EMIT_MAX_TILES_M = 16, EMIT_MAX_PARTS = 24;
-static EmitScratch* emit_scratch(cudaStream_t stream) {
-  // one scratch per (device, stream): LayerNorm-emitting launches of different streams (two host threads driving the model,
-  // as the reference's SLAM worker does, slam.py:533) must not share counters.  Entries live for the process lifetime.
-  static std::mutex mu;
-  static std::map<std::pair<int, cudaStream_t>, EmitScratch> table;
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return nullptr;
-  std::lock_guard<std::mutex> lock(mu);
-  EmitScratch& e = table[std::make_pair(dev, stream)];
-  if (!e.stats) {
-    void* a = nullptr; void* b = nullptr;
-    if (cudaMalloc(&a, sizeof(float2) * EMIT_MAX_TILES_M * EMIT_MAX_PARTS * BM) != cudaSuccess) return nullptr;
-    if (cudaMalloc(&b, sizeof(unsigned int) * 2 * EMIT_MAX_TILES_M) != cudaSuccess) { cudaFree(a); return nullptr; }
-    if (cudaMemset(b, 0, sizeof(unsigned int) * 2 * EMIT_MAX_TILES_M) != cudaSuccess) { cudaFree(a); cudaFree(b); return nullptr; }
-    void* c = nullptr; void* d = nullptr;
-    if (cudaMalloc(&c, sizeof(float) * EMIT_MAX_KSPLIT_TILES * BM * 64) != cudaSuccess) { cudaFree(a); cudaFree(b); return nullptr; }
-    if (cudaMalloc(&d, sizeof(unsigned int) * EMIT_MAX_KSPLIT_TILES) != cudaSuccess || cudaMemset(d, 0, sizeof(unsigned int) * EMIT_MAX_KSPLIT_TILES) != cudaSuccess) {
-      cudaFree(a); cudaFree(b); cudaFree(c); return nullptr;
-    }
-    e.stats = reinterpret_cast<float2*>(a); e.sync = reinterpret_cast<unsigned int*>(b);
-    e.kpart = reinterpret_cast<float4*>(c); e.kflag = reinterpret_cast<unsigned int*>(d);
+static const StreamState* emit_scratch(cudaStream_t stream) {
+  RegistryLock lock;
+  StreamState* st = stream_state(stream, lock);
+  if (!st || st->emit_stats) return st;
+  void *a = nullptr, *b = nullptr, *c = nullptr, *d = nullptr;
+  const size_t sync_bytes = sizeof(unsigned int) * 2 * EMIT_MAX_TILES_M, kflag_bytes = sizeof(unsigned int) * EMIT_MAX_KSPLIT_TILES;
+  // the kernels rely on the counters starting at zero: clear them in order with the launches that will use them
+  if (cudaMalloc(&a, sizeof(float2) * EMIT_MAX_TILES_M * EMIT_MAX_PARTS * BM) != cudaSuccess ||
+      cudaMalloc(&b, sync_bytes) != cudaSuccess || cudaMemsetAsync(b, 0, sync_bytes, stream) != cudaSuccess ||
+      cudaMalloc(&c, sizeof(float) * EMIT_MAX_KSPLIT_TILES * BM * 64) != cudaSuccess ||
+      cudaMalloc(&d, kflag_bytes) != cudaSuccess || cudaMemsetAsync(d, 0, kflag_bytes, stream) != cudaSuccess) {
+    cudaFree(a); cudaFree(b); cudaFree(c); cudaFree(d);
+    return nullptr;
   }
-  return &e;
+  st->emit_stats = reinterpret_cast<float2*>(a); st->emit_sync = reinterpret_cast<unsigned int*>(b);
+  st->emit_kpart = reinterpret_cast<float4*>(c); st->emit_kflag = reinterpret_cast<unsigned int*>(d);
+  return st;
 }
 
 template <int BN, int MODE>
@@ -563,22 +554,14 @@ static int launch_gemm(const m3r_gemm_args* a, cudaStream_t stream, const m3r_ge
     }
   }
   if constexpr (MODE == MODE_EMIT) {
-    EmitScratch* e = emit_scratch(stream);
+    const StreamState* e = emit_scratch(stream);
     if (!e) return set_error("gemm: LayerNorm-emit scratch allocation failed");
-    p.norm_out = a->norm_out; p.ldn = a->ldn; p.norm_eps = a->norm_eps; p.stats = e->stats; p.sync = e->sync;
-    static int ks_env = -1;
-    if (ks_env < 0) { const char* v = getenv("M3R_KSPLIT"); ks_env = (v && v[0] == '0') ? 0 : 1; }
-    if (BN == 64 && ks_env && a->K >= 2048 && (a->K / BK) % 2 == 0 && 2 * tiles <= num_sms() && tiles <= EMIT_MAX_KSPLIT_TILES) {
-      p.ksplit = 2; p.kpart = e->kpart; p.kflag = e->kflag;
+    p.norm_out = a->norm_out; p.ldn = a->ldn; p.norm_eps = a->norm_eps; p.stats = e->emit_stats; p.sync = e->emit_sync;
+    if (BN == 64 && a->K >= 2048 && (a->K / BK) % 2 == 0 && 2 * tiles <= num_sms() && tiles <= EMIT_MAX_KSPLIT_TILES) {
+      p.ksplit = 2; p.kpart = e->emit_kpart; p.kflag = e->emit_kflag;
     }
   }
-  static bool attr_set[64] = {};
-  int dev = 0; cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && !attr_set[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_kernel<BN, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES_PEER);
-    if (e != cudaSuccess) return set_error("gemm: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-    attr_set[dev] = true;
-  }
+  if (kernel_setup((const void*)gemm_kernel<BN, MODE>, Cfg::SMEM_BYTES_PEER, GEMM_THREADS).resident == 0) return 1;
   int grid = tiles < num_sms() ? tiles : num_sms();
   if (MODE == MODE_EMIT) grid = tiles * p.ksplit;
   if (MODE == MODE_GROUPED && grp->max_ctas > 0 && grid > grp->max_ctas) grid = grp->max_ctas;

@@ -110,51 +110,37 @@ extern "C" int m3r_encoder_forward(const m3r_encoder_weights* w, const float* im
 // ------------------------------------------------------------------------------------------------ decoder
 namespace m3r {
 
-// Side streams, one set per device: `s` runs the feedback MLP and the memory append (post-feedback K|V of every level)
-// concurrently with the last decoder block and the head; `copy` moves the old memory rows when the caller wants a fresh
-// concatenated tensor.  Fork / join with events; M3R_SIDE_STREAM=0 disables them.
-struct SideStream {
-  cudaStream_t s = nullptr, copy = nullptr;
-  cudaEvent_t ev[32];
-  int next = 0;
-  bool ok = false, enabled = true;
-  void init() {
-    if (ok || !enabled) return;
-    const char* e = getenv("M3R_SIDE_STREAM");
-    if (e && e[0] == '0') { enabled = false; return; }
-    if (cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) != cudaSuccess) { enabled = false; return; }
-    if (cudaStreamCreateWithFlags(&copy, cudaStreamNonBlocking) != cudaSuccess) { enabled = false; return; }
-    for (int i = 0; i < 32; ++i)
-      if (cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming) != cudaSuccess) { enabled = false; return; }
-    ok = true;
-  }
-  // make `to` wait for everything enqueued on `from` so far
-  int link(cudaStream_t from, cudaStream_t to) {
-    cudaEvent_t e = ev[next]; next = (next + 1) & 31;
-    cudaError_t r = cudaEventRecord(e, from);
-    if (r == cudaSuccess) r = cudaStreamWaitEvent(to, e, 0);
-    return r == cudaSuccess ? 0 : set_error("decoder_forward: stream fork/join failed: %s", cudaGetErrorString(r));
-  }
-};
+// The side streams of caller stream `cs` (StreamState::side / copy and their events), created on its first update call.
+// They belong to the caller's stream: host threads that drive the model on their own streams never wait on each other.
+static StreamState* side_streams_of(cudaStream_t cs) {
+  RegistryLock lock;
+  StreamState* st = stream_state(cs, lock);
+  if (!st) return set_error("decoder_forward: no current device"), nullptr;
+  if (st->side) return st;                                      // created last: the set is complete
+  cudaError_t e = st->copy ? cudaSuccess : cudaStreamCreateWithFlags(&st->copy, cudaStreamNonBlocking);
+  for (int i = 0; i < 32 && e == cudaSuccess; ++i) if (!st->ev[i]) e = cudaEventCreateWithFlags(&st->ev[i], cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&st->side, cudaStreamNonBlocking);
+  return e == cudaSuccess ? st : (set_error("decoder_forward: side stream creation failed: %s", cudaGetErrorString(e)), nullptr);
+}
+// make `to` wait for everything enqueued on `from` so far
+static int link(StreamState* st, cudaStream_t from, cudaStream_t to) {
+  cudaEvent_t e = st->ev[st->next_ev]; st->next_ev = (st->next_ev + 1) & 31;
+  cudaError_t r = cudaEventRecord(e, from);
+  if (r == cudaSuccess) r = cudaStreamWaitEvent(to, e, 0);
+  return r == cudaSuccess ? 0 : set_error("decoder_forward: stream fork/join failed: %s", cudaGetErrorString(r));
+}
 // Joins whatever was forked onto the side / copy streams when the enclosing call returns early (an M3R_TRY error path):
 // the caller's stream must never be left without a dependency on work that touches its buffers.
 struct SideJoin {
-  SideStream* sd = nullptr;
+  StreamState* sd = nullptr;
   cudaStream_t cs = nullptr;
   bool forked = false, copying = false, done = false;
   ~SideJoin() {
     if (done || !sd) return;
-    if (forked) sd->link(sd->s, cs);
-    if (copying) sd->link(sd->copy, cs);
+    if (forked) link(sd, sd->side, cs);
+    if (copying) link(sd, sd->copy, cs);
   }
 };
-
-static SideStream* side_streams() {
-  static SideStream per_dev[64];
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return nullptr;
-  return &per_dev[dev];
-}
 
 struct DecWs {
   uint16_t *enc16, *h16, *big16, *q16, *att16, *mlp16, *kvnew;
@@ -264,20 +250,19 @@ extern "C" int m3r_decoder_forward(const m3r_decoder_weights* w, const m3r_decod
   // (context parallel: the scene's memory is non-empty even when this rank's shard is)
   const bool use_skip = !c->render && (Nm > 0 || n_total > 1 || cp);
   if (cp && c->cp_slot_bytes < m3r_decoder_cp_slot_bytes(w, M)) return set_error("decoder_forward: cp_slot_bytes too small");
-  SideStream* sd = store_new ? side_streams() : nullptr;
-  if (sd) sd->init();
-  const bool side = sd && sd->ok;
+  StreamState* sd = nullptr;
+  if (store_new && !(sd = side_streams_of(cs))) return 1;
   SideJoin join_guard;
-  if (side) { join_guard.sd = sd; join_guard.cs = cs; }
+  join_guard.sd = sd; join_guard.cs = cs;
   if (store_new && Nm > 0 && !c->new_only) {
     // old memory rows -> output memory tensors (the reference's torch.cat, decoder.py:330) unless the caller appends in
     // place (mem_out[l] == mem[l]); independent of the whole step: copy stream, joined at the end
-    cudaStream_t cps = side ? sd->copy : cs;
+    cudaStream_t cps = sd->copy;
     bool linked = false;
     for (int l = 0; l < depth; ++l) {
       if (!c->mem_out[l]) return set_error("decoder_forward: mem_out[%d] is null", l);
       if (c->mem[l] == c->mem_out[l]) continue;
-      if (side && !linked) { M3R_TRY(sd->link(cs, cps)); linked = true; join_guard.copying = true; }
+      if (!linked) { M3R_TRY(link(sd, cs, cps)); linked = true; join_guard.copying = true; }
       cudaError_t e = cudaSuccess;
       if (c->mem_bstride_rows == 0 && B > 1) {            // stride-0 (expanded) memory: one source block for every scene
         for (int bb = 0; bb < B && e == cudaSuccess; ++bb)
@@ -293,10 +278,8 @@ extern "C" int m3r_decoder_forward(const m3r_decoder_weights* w, const m3r_decod
 
   // LayerNorm placement: when the [M, D] residual stream fits in one wave of 128x64 tiles, every GEMM that produces it
   // also emits the normalised rows for its consumer (m3r_gemm_args.norm_out); otherwise a separate affine-free pass runs.
-  static int emit_env = -1;
-  if (emit_env < 0) { const char* e = getenv("M3R_EMIT"); emit_env = (e && e[0] == '0') ? 0 : 1; }
   const int tiles_m = (M + 127) / 128;
-  const bool emit = emit_env == 1 && D % 64 == 0 && D <= 768 && tiles_m <= 16 && tiles_m * (D / 64) <= num_sms();
+  const bool emit = D % 64 == 0 && D <= 768 && tiles_m <= 16 && tiles_m * (D / 64) <= num_sms();
   // residual-stream GEMM: xo = xr + A W^T + b, followed by (or fused with) the normalisation of xo into h16
   auto res_gemm = [&](const void* A, int64_t lda, const void* W, int K, const float* bias, const float* xr, float* xo,
                       const float* rowbias, int rb_period, int rb_first, int Mrows, int64_t row_off) -> int {
@@ -383,9 +366,8 @@ extern "C" int m3r_decoder_forward(const m3r_decoder_weights* w, const m3r_decod
         m3r_gemm_group grp = {};
         grp.groups = depth; grp.w_group_rows = 5 * D; grp.bias_group = 5 * D;
         // next to the main chain (side stream): leave the SMs a LayerNorm-emitting GEMM needs (one wave of 128x64 tiles)
-        static int cap_env = -1;
-        if (cap_env < 0) { const char* e = getenv("M3R_APPEND_CAP"); cap_env = (e && e[0] == '0') ? 0 : 1; }
-        if (st != stream && cap_env) { const int keep = tiles_m * (D / 64); const int left = num_sms() - keep; grp.max_ctas = left > 32 ? left : 32; }
+        const int left = num_sms() - tiles_m * (D / 64);
+        grp.max_ctas = left > 32 ? left : 32;
         a.A = ws.hpost16; a.W = reinterpret_cast<const uint16_t*>(w->blocks[0].a_w) + (int64_t)3 * D * D; a.bias = w->blocks[0].a_b + 3 * D;
         for (int l = 0; l < depth; ++l) {
           grp.out[l] = reinterpret_cast<uint16_t*>(c->mem_out[l]) + orow * 2 * D;
@@ -410,10 +392,9 @@ extern "C" int m3r_decoder_forward(const m3r_decoder_weights* w, const m3r_decod
   auto maybe_append = [&](int ready_level) -> int {      // called when X_{ready_level} has been enqueued
     if (!store_new || appended || ready_level != depth - 1) return 0;
     appended = true;
-    if (!side) return 0;                                  // without a side stream the append runs after the head
-    M3R_TRY(sd->link(cs, sd->s));
+    M3R_TRY(link(sd, cs, sd->side));
     join_guard.forked = true;
-    return append_memory(sd->s);
+    return append_memory(sd->side);
   };
   M3R_TRY(maybe_append(0));
 
@@ -526,11 +507,8 @@ extern "C" int m3r_decoder_forward(const m3r_decoder_weights* w, const m3r_decod
   }
 
   if (store_new) {
-    if (!side) M3R_TRY(append_memory(stream));
-    if (side) {
-      M3R_TRY(sd->link(sd->s, cs));                                // join the side stream
-      if (Nm > 0 && !c->new_only) M3R_TRY(sd->link(sd->copy, cs));  // and the old-memory copies
-    }
+    M3R_TRY(link(sd, sd->side, cs));                                // join the side stream
+    if (Nm > 0 && !c->new_only) M3R_TRY(link(sd, sd->copy, cs));    // and the old-memory copies
   }
   join_guard.done = true;
   return 0;

@@ -1,8 +1,10 @@
-// Runtime glue of libm3r_b200.so: error reporting, device queries, TMA descriptor encoding.
+// Runtime glue of libm3r_b200.so: error reporting, the per-device / per-stream state registry, TMA descriptor encoding.
 #include <stdarg.h>
 #include <stdio.h>
 #include <string.h>
 #include <atomic>
+#include <map>
+#include <utility>
 #include <vector>
 #include "m3r_internal.h"
 
@@ -21,12 +23,6 @@ int set_error(const char* fmt, ...) {
 
 static unsigned long long* g_trace = nullptr;
 unsigned long long* trace_buffer() { return g_trace; }
-
-bool pdl_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("M3R_PDL"); v = (e && e[0] == '0') ? 0 : 1; }
-  return v == 1;
-}
 
 void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 
@@ -48,15 +44,46 @@ ProfScope::ProfScope(int cat, double flops, double bytes, cudaStream_t s) : slot
 }
 ProfScope::~ProfScope() { if (slot >= 0) cudaEventRecord(g_prof[slot].b, stream); }
 
+// ---- the registry (m3r_internal.h)
+struct DeviceState { int sms = 0; std::map<const void*, KernelInfo> kernels; };
+static std::mutex g_mu;
+static std::map<int, DeviceState> g_devices;
+static std::map<std::pair<int, cudaStream_t>, StreamState> g_streams;
+
 int num_sms() {
-  static int sms[64] = {};                      // per device
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
-  if (sms[dev] == 0) {
-    cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev);
-    if (sms[dev] <= 0) sms[dev] = 132;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+  std::lock_guard<std::mutex> lock(g_mu);
+  int& n = g_devices[dev].sms;
+  if (n <= 0 && (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)) n = 132;
+  return n;
+}
+
+KernelInfo kernel_setup(const void* fn, size_t smem_bytes, int threads) {
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return set_error("kernel setup: no current device: %s", cudaGetErrorString(e)), KernelInfo{};
+  std::lock_guard<std::mutex> lock(g_mu);
+  KernelInfo& k = g_devices[dev].kernels[fn];
+  if (k.resident == 0) {
+    cudaFuncAttributes fa;
+    int n = 0;
+    e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
+    if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, fn);
+    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn, threads, smem_bytes);
+    if (e != cudaSuccess || n < 1)
+      return set_error("kernel setup (%zu B shared memory, %d threads): %s", smem_bytes, threads,
+                       e != cudaSuccess ? cudaGetErrorString(e) : "no CTA fits on an SM"), KernelInfo{};
+    k.regs = fa.numRegs; k.resident = n;
   }
-  return sms[dev];
+  return k;
+}
+
+StreamState* stream_state(cudaStream_t s, RegistryLock& lock) {
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return nullptr;
+  lock = RegistryLock(g_mu);
+  return &g_streams[std::make_pair(dev, s)];
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,

@@ -444,8 +444,7 @@ ENCODE_AHEAD_BATCH = 50
 
 def _encode_missing_upfront(encoder, imgs, true_shape, x, pos, device, max_bs=None):
     """Fill x / pos for every view whose features are missing, in batches of views with one true_shape (CUDA encoder only)."""
-    import os
-    if not str(device).startswith("cuda") or not getattr(encoder, "batches_well", False) or os.environ.get("M3R_ENCODE_AHEAD", "1") == "0":
+    if not str(device).startswith("cuda") or not getattr(encoder, "batches_well", False):
         return
     missing = [i for i in range(len(x)) if x[i] is None or pos[i] is None]
     if len(missing) < 2:

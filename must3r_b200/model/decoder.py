@@ -356,7 +356,7 @@ class MUSt3R(nn.Module):
                 call.n_peers, call.peer_mem = len(_peer_ptrs), flat
                 keep.append(flat)
         nbytes = lib.m3r_decoder_workspace_bytes(C.byref(w), C.byref(call))
-        with torch.cuda.device(dev):           # the library keys its per-device state (side streams, scratch) on the current device
+        with torch.cuda.device(dev):           # the library keys its per-stream state (side streams, scratch) on the current device
             ws = cm.workspace(dev, nbytes, "dec")
             _lib.check(lib.m3r_decoder_forward(C.byref(w), C.byref(call), C.c_void_p(ws.data_ptr()), ws.numel(), cm.stream_ptr(dev)),
                        "decoder_forward")

@@ -354,8 +354,8 @@ def test_stream_schedule_inplace_memory_equals_copy_path():
 
 def test_two_host_threads_on_two_streams():
     """The reference's SLAM drives the model from a worker thread while another thread owns the main stream (slam.py:533): two
-    host threads running decoder chains at the same time on their own CUDA streams (per-stream workspaces, LayerNorm-emit
-    counters and attention split scratch) must reproduce the single-threaded results bit for bit (tools/two_threads.py)."""
+    host threads running decoder chains at the same time on their own CUDA streams (per-stream workspaces, side streams and
+    their events, LayerNorm-emit counters and attention split scratch) must reproduce the single-threaded results bit for bit (tools/two_threads.py)."""
     import subprocess
     import sys
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

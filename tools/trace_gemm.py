@@ -9,7 +9,6 @@ from must3r_b200 import ops, _lib  # noqa: E402
 
 M, N, K = (int(v) for v in sys.argv[1:4]) if len(sys.argv) > 3 else (768, 768, 768)
 if len(sys.argv) > 4: os.environ["M3R_GEMM_BN"] = sys.argv[4]
-os.environ["M3R_GEMM_PAIR"] = "0"
 dt = torch.bfloat16
 a = torch.randn(M, K, device="cuda").to(dt); w = torch.randn(N, K, device="cuda").to(dt)
 bias = torch.randn(N, device="cuda"); res = torch.randn(M, N, device="cuda")
