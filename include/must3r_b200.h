@@ -223,6 +223,20 @@ int m3r_postprocess(const float* pm, int64_t P, float* pts3d, float* pts3d_local
  * (must3r/slam/nns.py:57-62, called from must3r/slam/model.py:82). */
 int m3r_nn_min_dist(const float* queries, int32_t Q, const float* db, int64_t P, float* out, void* stream);
 
+/* Exact nearest-neighbour grid index over a point map with per-point buckets (the viewing-direction quadrants of
+ * must3r/slam/nns.py:65-95 QuandrantSearcher, or one bucket for KDTree_scipy).  Cells are cubes of side h.
+ * m3r_pointgrid_keys: keys[i] = 64-bit sort key of pts[i] [P,3] fp32 with bucket[i] (int32 in [0, 512), NULL = all 0):
+ * the bucket, then the Morton code of the cell floor(pts * inv_h); points whose cell is out of the key range or non-finite get
+ * the bucket's overflow key, which sorts after all its cells.  The caller sorts the points by key and builds
+ * pts [P,3] (sorted), cell_keys [C] (the distinct sorted keys), cell_off [C+1] int32 (point range of each cell) and
+ * bucket_cells [nb+1] int32 (cell range of each bucket).
+ * m3r_pointgrid_query: out[i] = distance from queries[i] to the nearest point of bucket qbucket[i] (NULL = all 0), inf if
+ * that bucket is empty; bitwise equal to m3r_nn_min_dist over that bucket's points. */
+int m3r_pointgrid_keys(const float* pts, const int32_t* bucket, int64_t P, float inv_h, int64_t* keys, void* stream);
+int m3r_pointgrid_query(const float* queries, const int32_t* qbucket, int32_t Q, const float* pts, int64_t P,
+                        const int64_t* cell_keys, const int32_t* cell_off, int32_t C, const int32_t* bucket_cells,
+                        int32_t nb, float h, float inv_h, float* out, void* stream);
+
 /* ---------------------------------------------------------------------------------------------------
  * Input preprocessing of V RGB uint8 frames of one size: src [V, src_h, src_w, 3] uint8 (HWC; pixel stride 3 bytes,
  * row pitch src_pitch bytes, frame stride src_vstride bytes - a crop view or a padded frame needs no copy) -> fp32

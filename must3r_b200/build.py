@@ -13,7 +13,7 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libm3r_b200.so")
-SOURCES = ["runtime.cu", "elementwise.cu", "gemm.cu", "attention.cu", "model.cu", "image.cu"]  # missing files are skipped
+SOURCES = ["runtime.cu", "elementwise.cu", "gemm.cu", "attention.cu", "model.cu", "image.cu", "pointgrid.cu"]  # missing files are skipped
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = GENCODE + ["-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC"]

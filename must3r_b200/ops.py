@@ -305,6 +305,31 @@ def resize_aa_bilinear_u8(src: torch.Tensor, tables, xk: int, yk: int, out_hw, t
                                                     yk, oh, _p(tmp), _p(out), _stream()), "resize_aa_bilinear_u8")
 
 
+def pointgrid_keys(pts: torch.Tensor, bucket: Optional[torch.Tensor], inv_h: float) -> torch.Tensor:
+    """Grid-index sort keys of pts [P,3] fp32 with int32 buckets [P] (None = all 0): [P] int64 (csrc/pointgrid.cu)."""
+    _req_cuda(pts, bucket)
+    assert pts.dtype == torch.float32 and pts.is_contiguous() and pts.shape[-1] == 3
+    assert bucket is None or (bucket.dtype == torch.int32 and bucket.is_contiguous() and bucket.numel() == pts.shape[0])
+    keys = torch.empty((pts.shape[0],), dtype=torch.int64, device=pts.device)
+    _lib.check(_lib.lib().m3r_pointgrid_keys(_p(pts), _p(bucket), pts.shape[0], inv_h, _p(keys), _stream()), "pointgrid_keys")
+    return keys
+
+
+def pointgrid_query(queries: torch.Tensor, qbucket: Optional[torch.Tensor], pts: torch.Tensor, cell_keys: torch.Tensor,
+                    cell_off: torch.Tensor, bucket_cells: torch.Tensor, h: float, inv_h: float) -> torch.Tensor:
+    """Distance from each query [Q,3] fp32 to the nearest indexed point of its bucket (int32 [Q], None = all 0): [Q] fp32,
+    inf for an empty bucket.  The index tensors are those m3r_pointgrid_query documents (engine/keyframes.py builds them)."""
+    _req_cuda(queries, qbucket, pts, cell_keys, cell_off, bucket_cells)
+    assert queries.dtype == torch.float32 and queries.is_contiguous() and queries.shape[-1] == 3
+    assert qbucket is None or (qbucket.dtype == torch.int32 and qbucket.is_contiguous() and qbucket.numel() == queries.shape[0])
+    assert cell_keys.dtype == torch.int64 and cell_off.dtype == torch.int32 and bucket_cells.dtype == torch.int32
+    out = torch.empty((queries.shape[0],), dtype=torch.float32, device=queries.device)
+    _lib.check(_lib.lib().m3r_pointgrid_query(_p(queries), _p(qbucket), queries.shape[0], _p(pts), pts.shape[0], _p(cell_keys),
+                                              _p(cell_off), cell_keys.shape[0], _p(bucket_cells), bucket_cells.shape[0] - 1,
+                                              h, inv_h, _p(out), _stream()), "pointgrid_query")
+    return out
+
+
 def postprocess_raw(pm: torch.Tensor):
     _req_cuda(pm)
     assert pm.dtype == torch.float32 and pm.shape[-1] == 7
