@@ -3,9 +3,11 @@
 //   warps 0..7 : two consumer warpgroups -- warpgroup w multiplies rows [64w, 64w + 64) of the 128-row tile with
 //                wgmma.m64nBNk16 (operands straight from the 128B-swizzled smem ring, fp32 accumulator in registers),
 //                then runs the epilogue: bias / RoPE / GELU / residual / image2-embed row bias, vectorised global stores
-//   warp 8     : TMA producer (one elected lane) -- A and W tiles, 128B-swizzled, mbarrier ring
+//   warps 8..11: producer warpgroup -- one elected lane issues TMA (A and W tiles, 128B-swizzled, mbarrier ring); the
+//                warpgroup gives its registers to the consumers (setmaxnreg), whose accumulator is 128 registers at BN = 256
 // The producer keeps filling the ring for the next tile while the consumers drain the current one.  Tiles are walked
-// m-fastest so that co-resident CTAs share the weight tile in L2.
+// m-fastest so that co-resident CTAs share the weight tile in L2.  The operand type (fp16 / bf16) is a template parameter:
+// a run-time choice between two wgmma forms inside the k loop makes ptxas fence the accumulator between wgmma groups.
 #include "ptx.cuh"
 #include "m3r_internal.h"
 
@@ -14,24 +16,35 @@ namespace m3r {
 constexpr int BM = 128;
 constexpr int BK = 64;        // 64 x 16-bit = 128 B = one swizzle atom
 constexpr int MMA_K = 16;
-constexpr int GEMM_THREADS = 288;      // 2 consumer warpgroups + the TMA warp
-constexpr int PRODUCER_WARP = 8;
+constexpr int GEMM_THREADS = 384;      // 2 consumer warpgroups + the producer warpgroup
+constexpr int PRODUCER_WARP = 8;       // first warp of the producer warpgroup
 constexpr int SMEM_MAX = 232448;       // 227 KB: the most dynamic shared memory an sm_90 block may opt in to
+// Register split after setmaxnreg.  The warpgroups can only redistribute what the CTA was given at launch (the
+// __launch_bounds__ cap, 168 x 384 threads): an increase the CTA cannot cover would wait forever.
+constexpr int GEMM_LAUNCH_REGS = (65536 / GEMM_THREADS) / 8 * 8;
+constexpr int GEMM_PRODUCER_REGS = 40;
+constexpr int GEMM_CONSUMER_REGS = 232;
+static_assert(128 * GEMM_PRODUCER_REGS + 256 * GEMM_CONSUMER_REGS <= GEMM_LAUNCH_REGS * GEMM_THREADS,
+              "register split exceeds the launch allocation");
 
 template <int BN>
 struct GemmCfg {
   static constexpr int STAGE_BYTES = (BM + BN) * BK * 2;
   static constexpr int STG_BYTES = 2 * 2 * 64 * 33 * 4;        // epilogue transpose: [warpgroup][chunk][64 rows][33]
   static constexpr int PEER_STAGE_BYTES = 8 * 4096;          // per consumer warp 32 rows x 128 B: transposes peer stores (below)
-  static constexpr int FIXED = 1024 /*align*/ + 256 /*barriers*/ + STG_BYTES + PEER_STAGE_BYTES;
-  static constexpr int STAGES = (SMEM_MAX - FIXED) / STAGE_BYTES;   // 256:3  192:4  160:4  128:5  64:6  32:8
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256 + STG_BYTES;
-  static constexpr int SMEM_BYTES_PEER = SMEM_BYTES + PEER_STAGE_BYTES;
+  static constexpr int FIXED = 1024 /*align*/ + 256 /*barriers*/ + STG_BYTES;
+  // Only launches that store to peers reserve the peer transpose tile; the others spend that space on the operand ring.
+  static constexpr int STAGES = (SMEM_MAX - FIXED) / STAGE_BYTES;                           // 256:4  192:4  160:5  128:6  64:8  32:9
+  static constexpr int STAGES_PEER = (SMEM_MAX - FIXED - PEER_STAGE_BYTES) / STAGE_BYTES;   // 256:3  192:4  160:4  128:5  64:6  32:8
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + FIXED;
+  static constexpr int SMEM_BYTES_PEER = STAGES_PEER * STAGE_BYTES + FIXED + PEER_STAGE_BYTES;
+  static constexpr int SMEM_BYTES_MAX = SMEM_BYTES > SMEM_BYTES_PEER ? SMEM_BYTES : SMEM_BYTES_PEER;
+  static_assert(2 * STAGES * 8 <= 256, "ring barriers exceed their space");
 };
 
 struct GemmParams {
   int M, N, K;
-  int is_bf16;
+  int stages;                  // depth of the operand ring: GemmCfg::STAGES, or STAGES_PEER when the peer tile is reserved
   const float* bias;
   int act;
   const float* residual;
@@ -130,6 +143,7 @@ __device__ __forceinline__ void epilogue_math(const GemmParams& p, const float* 
 // Store of one chunk: fp32 or 16-bit row segment; the 16-bit form optionally also goes to the peers' buffers.
 // A peer store instruction of a warp covers 32 rows x 16 B; the four uint4 of a thread complete a 64-byte segment per
 // row back to back, so NVLink sees 64 B write bursts (the fused GEMM -> all-gather path).
+template <bool BF16>
 __device__ __forceinline__ void epilogue_store(const GemmParams& p, void* out, void* const* peers, const float (&v)[32], long long orow, int col0) {
   if (p.out_dtype == 0) {
     float4* o4 = reinterpret_cast<float4*>(reinterpret_cast<float*>(out) + orow * p.ldc + col0);
@@ -139,10 +153,10 @@ __device__ __forceinline__ void epilogue_store(const GemmParams& p, void* out, v
     uint4 w[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      w[i].x = pack16(v[8 * i], v[8 * i + 1], p.is_bf16);
-      w[i].y = pack16(v[8 * i + 2], v[8 * i + 3], p.is_bf16);
-      w[i].z = pack16(v[8 * i + 4], v[8 * i + 5], p.is_bf16);
-      w[i].w = pack16(v[8 * i + 6], v[8 * i + 7], p.is_bf16);
+      w[i].x = pack16(v[8 * i], v[8 * i + 1], BF16);
+      w[i].y = pack16(v[8 * i + 2], v[8 * i + 3], BF16);
+      w[i].z = pack16(v[8 * i + 4], v[8 * i + 5], BF16);
+      w[i].w = pack16(v[8 * i + 6], v[8 * i + 7], BF16);
     }
     uint4* o4 = reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(out) + orow * p.ldc + col0);
 #pragma unroll
@@ -153,13 +167,6 @@ __device__ __forceinline__ void epilogue_store(const GemmParams& p, void* out, v
       for (int i = 0; i < 4; ++i) q4[i] = w[i];
     }
   }
-}
-
-__device__ __forceinline__ void epilogue_chunk(const GemmParams& p, const uint32_t (&raw)[32], int row, bool row_ok, long long orow,
-                                               bool rb_on, const float* rope_row, int col0) {
-  float v[32];
-  epilogue_math(p, p.bias, raw, v, row, row_ok, rb_on, rope_row, col0);
-  if (row_ok) epilogue_store(p, p.out, p.peer_out, v, orow, col0);
 }
 
 __device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int* p) {
@@ -178,12 +185,12 @@ struct NoTab {};
 template <int MODE> struct TabOf { using type = NoTab; };
 template <> struct TabOf<MODE_GROUPED> { using type = GemmGroupTab; };
 
-template <int BN, int MODE>
+template <int BN, int MODE, bool BF16>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW, const GemmParams p,
             const __grid_constant__ typename TabOf<MODE>::type tab) {
   using Cfg = GemmCfg<BN>;
-  constexpr int STAGES = Cfg::STAGES;
+  const int STAGES = p.stages;
   constexpr int NCHUNK = BN / 32;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -222,9 +229,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   __syncthreads();
   M3R_TR(if (tr && threadIdx.x == 0) tr[1] = gtime_ns();)
 
-  if (warp == PRODUCER_WARP) {
-    // ------------------------------------------------------------ TMA producer
-    if (elect_one()) {
+  if (warp >= PRODUCER_WARP) {
+    // ------------------------------------------------------------ TMA producer warpgroup
+    setmaxnreg_dec<GEMM_PRODUCER_REGS>();
+    if (warp == PRODUCER_WARP && elect_one()) {
       // The weights never depend on the kernel before this one, so the W halves of the first ring of stages are requested
       // BEFORE the programmatic-dependency wait: their (cold, HBM) latency overlaps the predecessor's tail.  The
       // activations follow after the wait; each stage's barrier expects both halves.
@@ -266,6 +274,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   }
 
   // ------------------------------------------------------------ consumer warpgroups 0, 1: wgmma + epilogue
+  setmaxnreg_inc<GEMM_CONSUMER_REGS>();
   griddep_wait();
   griddep_launch();
   const int wg = warp >> 2;                       // rows [64 wg, 64 wg + 64) of the tile
@@ -291,8 +300,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 #pragma unroll
       for (int k = 0; k < BK / MMA_K; ++k) {
         // advance 16 elements (32 bytes) along K inside the 128B swizzle atom: +2 in the >>4 address field
-        if (p.is_bf16) Wgmma<BN, true>::ss(acc, adesc + 2 * k, bdesc + 2 * k, 1);
-        else Wgmma<BN, false>::ss(acc, adesc + 2 * k, bdesc + 2 * k, 1);
+        Wgmma<BN, BF16>::ss(acc, adesc + 2 * k, bdesc + 2 * k, 1);
       }
       wgmma_commit();
       wgmma_wait<1>();                            // the previous k-block's MMAs are done: its stage may be refilled
@@ -364,7 +372,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         }
         if (threadIdx.x == 0) {
           unsigned int spins = 0;
-          while (ld_acquire_u32(p.kflag + t) == 0u) { if (++spins > (1u << 26)) __trap(); }
+          while (ld_acquire_u32(p.kflag + t) == 0u) { if (++spins > (1u << 26)) spin_timeout_trap(); }
           p.kflag[t] = 0u;                                    // re-armed for the next launch (nobody else touches it any more)
         }
         asm volatile("bar.sync 1, 256;" ::: "memory");
@@ -405,11 +413,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       // sit in front of the fence above)
       if (row_ok) {
 #pragma unroll
-        for (int pi = 0; pi < CPT; ++pi) epilogue_store(p, p.out, p.peer_out, v[pi], orow, n0 + (2 * pi + u) * 32);
+        for (int pi = 0; pi < CPT; ++pi) epilogue_store<BF16>(p, p.out, p.peer_out, v[pi], orow, n0 + (2 * pi + u) * 32);
       }
       if (threadIdx.x == 0) {
         unsigned int spins = 0;
-        while (ld_acquire_u32(cnt) < (unsigned int)tiles_n) { if (++spins > (1u << 26)) __trap(); }
+        while (ld_acquire_u32(cnt) < (unsigned int)tiles_n) { if (++spins > (1u << 26)) spin_timeout_trap(); }
       }
       asm volatile("bar.sync 1, 256;" ::: "memory");
       float msum = 0.f;
@@ -429,10 +437,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
             uint4 w;
-            w.x = pack16((v[pi][8 * i] - mean) * rstd, (v[pi][8 * i + 1] - mean) * rstd, p.is_bf16);
-            w.y = pack16((v[pi][8 * i + 2] - mean) * rstd, (v[pi][8 * i + 3] - mean) * rstd, p.is_bf16);
-            w.z = pack16((v[pi][8 * i + 4] - mean) * rstd, (v[pi][8 * i + 5] - mean) * rstd, p.is_bf16);
-            w.w = pack16((v[pi][8 * i + 6] - mean) * rstd, (v[pi][8 * i + 7] - mean) * rstd, p.is_bf16);
+            w.x = pack16((v[pi][8 * i] - mean) * rstd, (v[pi][8 * i + 1] - mean) * rstd, BF16);
+            w.y = pack16((v[pi][8 * i + 2] - mean) * rstd, (v[pi][8 * i + 3] - mean) * rstd, BF16);
+            w.z = pack16((v[pi][8 * i + 4] - mean) * rstd, (v[pi][8 * i + 5] - mean) * rstd, BF16);
+            w.w = pack16((v[pi][8 * i + 6] - mean) * rstd, (v[pi][8 * i + 7] - mean) * rstd, BF16);
             o4[i] = w;
           }
         }
@@ -463,8 +471,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
             uint4 w;
-            w.x = pack16(v[8 * i], v[8 * i + 1], p.is_bf16); w.y = pack16(v[8 * i + 2], v[8 * i + 3], p.is_bf16);
-            w.z = pack16(v[8 * i + 4], v[8 * i + 5], p.is_bf16); w.w = pack16(v[8 * i + 6], v[8 * i + 7], p.is_bf16);
+            w.x = pack16(v[8 * i], v[8 * i + 1], BF16); w.y = pack16(v[8 * i + 2], v[8 * i + 3], BF16);
+            w.z = pack16(v[8 * i + 4], v[8 * i + 5], BF16); w.w = pack16(v[8 * i + 6], v[8 * i + 7], BF16);
             if (row_ok) o4[i] = w;                                  // this GPU's copy: the thread's own row
             pst[lane * 8 + (i ^ (lane & 7))] = w;
           }
@@ -486,7 +494,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       } else if (cc < NCHUNK) {
         float v[32];
         epilogue_math(p, bias, raw, v, lrow, row_ok, rb_on, rope_row, n0 + cc * 32);
-        if (row_ok) epilogue_store(p, out_g, peers_g, v, orow, n0 + cc * 32);
+        if (row_ok) epilogue_store<BF16>(p, out_g, peers_g, v, orow, n0 + cc * 32);
       }
     }
     M3R_TR(if (tr && threadIdx.x == 0) tr[7] = gtime_ns();)
@@ -495,7 +503,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 }
 
 static void fill_params(GemmParams& p, const m3r_gemm_args* a) {
-  p.M = a->M; p.N = a->N; p.K = a->K; p.is_bf16 = a->is_bf16;
+  p.M = a->M; p.N = a->N; p.K = a->K;
   p.bias = a->bias; p.act = a->act; p.residual = a->residual; p.ldr = a->ldr;
   p.rowbias = a->rowbias; p.rb_period = a->rb_period > 0 ? a->rb_period : 1; p.rb_first = a->rb_first;
   p.rope_tab = a->rope_tab; p.rope_cols = a->rope_cols; p.rope_period = a->rope_period > 0 ? a->rope_period : 1;
@@ -561,7 +569,12 @@ static int launch_gemm(const m3r_gemm_args* a, cudaStream_t stream, const m3r_ge
       p.ksplit = 2; p.kpart = e->emit_kpart; p.kflag = e->emit_kflag;
     }
   }
-  if (kernel_setup((const void*)gemm_kernel<BN, MODE>, Cfg::SMEM_BYTES_PEER, GEMM_THREADS).resident == 0) return 1;
+  const auto kernel = a->is_bf16 ? gemm_kernel<BN, MODE, true> : gemm_kernel<BN, MODE, false>;
+  const KernelInfo k = kernel_setup((const void*)kernel, Cfg::SMEM_BYTES_MAX, GEMM_THREADS);
+  if (k.resident == 0) return 1;
+  if (k.regs < GEMM_LAUNCH_REGS) return set_error("gemm: kernel built with %d registers per thread, the register split needs %d", k.regs, GEMM_LAUNCH_REGS);
+  const bool peer_tile = a->n_peer_out > 0 && a->out_dtype != 0;
+  p.stages = peer_tile ? Cfg::STAGES_PEER : Cfg::STAGES;
   int grid = tiles < num_sms() ? tiles : num_sms();
   if (MODE == MODE_EMIT) grid = tiles * p.ksplit;
   if (MODE == MODE_GROUPED && grp->max_ctas > 0 && grid > grp->max_ctas) grid = grp->max_ctas;
@@ -569,8 +582,8 @@ static int launch_gemm(const m3r_gemm_args* a, cudaStream_t stream, const m3r_ge
   {
     const int cat = BN >= 256 ? PROF_GEMM256 : (BN >= 128 ? PROF_GEMM128 : PROF_GEMM64);
     ProfScope prof(cat, 2.0 * a->M * groups * (double)a->N * a->K, 2.0 * ((double)a->M * groups * a->K + (double)a->N * groups * a->K) + (double)a->M * groups * a->N * (a->out_dtype ? 2 : 4), stream);
-    const size_t smem_bytes = (a->n_peer_out > 0 && a->out_dtype != 0) ? Cfg::SMEM_BYTES_PEER : Cfg::SMEM_BYTES;
-    cudaError_t le = launch_pdl(gemm_kernel<BN, MODE>, dim3(grid), dim3(GEMM_THREADS), smem_bytes, stream, tmA, tmW, p, tab);
+    const size_t smem_bytes = peer_tile ? Cfg::SMEM_BYTES_PEER : Cfg::SMEM_BYTES;
+    cudaError_t le = launch_pdl(kernel, dim3(grid), dim3(GEMM_THREADS), smem_bytes, stream, tmA, tmW, p, tab);
     if (le != cudaSuccess) return set_error("gemm launch: %s", cudaGetErrorString(le));
   }
   cudaError_t e = cudaGetLastError();

@@ -62,11 +62,15 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
+// Ends a bounded spin that timed out.  Not inlined: a trap inside a loop makes ptxas allocate registers there against
+// the launch cap and ignore the larger budget of a setmaxnreg.inc region, so the consumers of a warp-specialised kernel
+// spill.
+static __device__ __noinline__ void spin_timeout_trap() { __trap(); }
 // Bounded wait: a protocol bug traps (reported as a launch failure) instead of hanging the GPU box.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (++spins > (1u << 28)) { __trap(); }
+    if (++spins > (1u << 28)) spin_timeout_trap();
   }
 }
 

@@ -1,6 +1,7 @@
 """Stand-alone timing of the attention / GEMM kernels at the shapes of the C3 job (CUDA events, L2 flushed between
-iterations by a 256 MB write).  `python tools/prof_attn.py [attn|gemm] [--once] [--compare]`; --once runs each shape twice
-for ncu; --compare also times each attention shape at the key-split count of the earlier rule (old_splits)."""
+iterations by a 256 MB write).  `python tools/prof_attn.py [attn|gemm] [--once] [--compare] [--fp16]`; --once runs each shape
+twice for ncu; --compare also times each attention shape at the key-split count of the earlier rule (old_splits); --fp16
+uses fp16 operands instead of bf16."""
 import os, sys, time
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -54,7 +55,7 @@ def old_splits(B, H, Nq, Nk, sms):
     return -(-key_tiles // chunk)
 
 
-dt = torch.bfloat16
+dt = torch.float16 if "--fp16" in sys.argv else torch.bfloat16
 if "attn" in which:
     for name, (B, H, Nq, Nk, grp) in {
         "render CA 20 views x M=20": (20, 12, 768, 15360, 20),
