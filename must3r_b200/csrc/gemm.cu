@@ -3,6 +3,7 @@
 //   warps 0..7 : two consumer warpgroups -- warpgroup w multiplies rows [64w, 64w + 64) of the 128-row tile with
 //                wgmma.m64nBNk16 (operands straight from the 128B-swizzled smem ring, fp32 accumulator in registers),
 //                then runs the epilogue: bias / RoPE / GELU / residual / image2-embed row bias, vectorised global stores
+//                (a CTA with several tiles: on the accumulator fragment, with TMA stores that drain during the next tile)
 //   warps 8..11: producer warpgroup -- one elected lane issues TMA (A and W tiles, 128B-swizzled, mbarrier ring); the
 //                warpgroup gives its registers to the consumers (setmaxnreg), whose accumulator is 128 registers at BN = 256
 // The producer keeps filling the ring for the next tile while the consumers drain the current one.  Tiles are walked
@@ -40,6 +41,9 @@ struct GemmCfg {
   static constexpr int SMEM_BYTES_PEER = STAGES_PEER * STAGE_BYTES + FIXED + PEER_STAGE_BYTES;
   static constexpr int SMEM_BYTES_MAX = SMEM_BYTES > SMEM_BYTES_PEER ? SMEM_BYTES : SMEM_BYTES_PEER;
   static_assert(2 * STAGES * 8 <= 256, "ring barriers exceed their space");
+  // the fragment-layout epilogue reuses the transpose area as 1024-aligned TMA store buffers: [warpgroup][2][64 rows x 128 B]
+  static constexpr int FRAG_STG_OFFSET = 1024, FRAG_BUF_BYTES = 64 * 128;
+  static_assert(FRAG_STG_OFFSET + 2 * 2 * FRAG_BUF_BYTES <= 256 + STG_BYTES, "store buffers exceed the epilogue area");
 };
 
 struct GemmParams {
@@ -62,6 +66,7 @@ struct GemmParams {
   void* peer_out[M3R_MAX_PEERS];
   unsigned long long* trace;   // debug only (m3r_debug_trace): 16 words per CTA; normally null
   int w_static;                // weights may be requested before the programmatic-dependency wait
+  int frag_epi;                // epilogue_frag + TMA stores through the output tensor map (persistent plain launches)
   // ---- grouped GEMM: `groups` independent problems of M rows each that share the shapes: A rows [g*M, (g+1)*M) of one
   // [groups*M, K] matrix, W rows [g*w_group_rows, +N), bias + g*bias_group, outputs from GemmGroupTab (groups == 1: `out`)
   int groups;
@@ -169,6 +174,124 @@ __device__ __forceinline__ void epilogue_store(const GemmParams& p, void* out, v
   }
 }
 
+// Epilogue of the persistent plain launches, applied to the accumulator fragment in place (no transpose through shared
+// memory).  Thread (warp w, lane l) of a consumer warpgroup holds rows 16w + l/4 and 16w + l/4 + 8 of the warpgroup's 64,
+// columns 8nb + 2(l%4) + {0, 1}; the RoPE partner of column c (c % 32 < 16) is column c + 16, block nb + 2 of the same
+// thread.  The per-element operations and their order are those of epilogue_math (bias, RoPE, row bias, GELU, residual),
+// so the results are bitwise the same.  Each 128-byte-wide column chunk (32 fp32 or 64 16-bit columns) is written into one
+// of the warpgroup's two staging buffers in the 128B-swizzled layout of the output tensor map (the fragment writes are
+// then free of bank conflicts) and leaves with one TMA store that neither the next chunk nor the next tile's MMAs wait for.
+// One barrier per chunk: its elected thread first waits until the previous chunk's store has read the other buffer.
+template <int BN, bool BF16, bool OUT16>
+__device__ __forceinline__ void epilogue_frag(const GemmParams& p, const CUtensorMap* tmC, float (&acc)[BN / 2], uint8_t* stg,
+                                              int row0, int n0, int wg, int ct) {
+  constexpr int CW = OUT16 ? 64 : 32;                // columns per store chunk
+  const int lane = ct & 31, q = lane & 3;
+  const int fr = (ct >> 5) * 16 + (lane >> 2);
+  const int sw = lane >> 2;                          // (row % 8) of both rows: the swizzle phase
+  bool row_ok[2], rb_on[2];
+  const float* rope_row[2];
+  const float* res_row[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int lrow = row0 + fr + 8 * h;
+    row_ok[h] = lrow < p.M;
+    rb_on[h] = p.rowbias != nullptr && (lrow % p.rb_period) >= p.rb_first;
+    rope_row[h] = p.rope_tab ? p.rope_tab + (long long)(lrow % p.rope_period) * 64 : nullptr;
+    res_row[h] = p.residual ? p.residual + (long long)lrow * p.ldr : nullptr;
+  }
+#pragma unroll
+  for (int sc = 0; sc < BN / CW; ++sc) {
+#pragma unroll
+    for (int c = sc * (CW / 32); c < (sc + 1) * (CW / 32); ++c) {
+      const int col0 = n0 + 32 * c;
+      if (p.bias) {
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+          const int nb = 4 * c + jj;
+          const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + 8 * nb + 2 * q));
+#pragma unroll
+          for (int h = 0; h < 2; ++h) { acc[4 * nb + 2 * h] += b.x; acc[4 * nb + 2 * h + 1] += b.y; }
+        }
+      }
+      if (p.rope_tab != nullptr && col0 < p.rope_cols) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (!row_ok[h]) continue;
+          const float* cs = rope_row[h] + ((col0 >> 5) & 1) * 32;
+#pragma unroll
+          for (int jj = 0; jj < 2; ++jj) {
+            const int i = 8 * jj + 2 * q;
+            const float2 c2 = __ldg(reinterpret_cast<const float2*>(cs + i));
+            const float2 s2 = __ldg(reinterpret_cast<const float2*>(cs + 16 + i));
+            const float cc[2] = {c2.x, c2.y}, ss[2] = {s2.x, s2.y};
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              float& vu = acc[4 * (4 * c + jj) + 2 * h + e];
+              float& vw = acc[4 * (4 * c + jj + 2) + 2 * h + e];
+              const float u = vu, w = vw;
+              vu = u * cc[e] - w * ss[e];
+              vw = w * cc[e] + u * ss[e];
+            }
+          }
+        }
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (!rb_on[h]) continue;
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+          const int nb = 4 * c + jj;
+          const float2 b = __ldg(reinterpret_cast<const float2*>(p.rowbias + n0 + 8 * nb + 2 * q));
+          acc[4 * nb + 2 * h] += b.x; acc[4 * nb + 2 * h + 1] += b.y;
+        }
+      }
+      if (p.act == 1) {
+#pragma unroll
+        for (int i = 16 * c; i < 16 * c + 16; ++i) acc[i] = gelu_erf(acc[i]);
+      }
+      if (p.residual) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (!row_ok[h]) continue;
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) {
+            const int nb = 4 * c + jj;
+            const float2 r = *reinterpret_cast<const float2*>(res_row[h] + n0 + 8 * nb + 2 * q);
+            acc[4 * nb + 2 * h] += r.x; acc[4 * nb + 2 * h + 1] += r.y;
+          }
+        }
+      }
+    }
+    // the chunk's 64 rows x 128 B, row r's 16-byte unit k at r * 128 + ((k ^ (r % 8)) << 4) (SWIZZLE_128B)
+    uint8_t* buf = stg + (sc & 1) * GemmCfg<BN>::FRAG_BUF_BYTES;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      uint8_t* rowp = buf + (fr + 8 * h) * 128;
+      if constexpr (OUT16) {
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const int nb = 8 * sc + jj;
+          *reinterpret_cast<uint32_t*>(rowp + ((jj ^ sw) << 4) + 4 * q) = pack16(acc[4 * nb + 2 * h], acc[4 * nb + 2 * h + 1], BF16);
+        }
+      } else {
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+          const int nb = 4 * sc + jj;
+          *reinterpret_cast<float2*>(rowp + (((2 * jj + (q >> 1)) ^ sw) << 4) + 8 * (q & 1)) = make_float2(acc[4 * nb + 2 * h], acc[4 * nb + 2 * h + 1]);
+        }
+      }
+    }
+    fence_proxy_async_smem();
+    if (ct == 0) bulk_wait_group_read<0>();          // the other buffer (next chunk) has been read by its store
+    asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+    if (ct == 0) {
+      tma_store_2d(tmC, buf, n0 + sc * CW, row0);
+      bulk_commit_group();
+    }
+  }
+}
+
 __device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int* p) {
   unsigned int v;
   asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
@@ -187,8 +310,8 @@ template <> struct TabOf<MODE_GROUPED> { using type = GemmGroupTab; };
 
 template <int BN, int MODE, bool BF16>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW, const GemmParams p,
-            const __grid_constant__ typename TabOf<MODE>::type tab) {
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
+            const __grid_constant__ CUtensorMap tmC, const GemmParams p, const __grid_constant__ typename TabOf<MODE>::type tab) {
   using Cfg = GemmCfg<BN>;
   const int STAGES = p.stages;
   constexpr int NCHUNK = BN / 32;
@@ -262,6 +385,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             tma_load_2d(sA + stage * BM * BK * 2, &tmA, &full[stage], (kb0 + kb) * BK, m0);
             tma_load_2d(sB + stage * BN * BK * 2, &tmW, &full[stage], (kb0 + kb) * BK, n0);
           }
+          if constexpr (MODE == MODE_PLAIN) {
+            // the tile's residual rows, spread over its k-blocks, go to L2 ahead of the epilogue's fragment-layout loads
+            if (p.frag_epi && p.residual) {
+              for (int r = kb; r < BM; r += num_kb)
+                if (m0 + r < p.M) prefetch_l2_bulk(p.residual + (long long)(m0 + r) * p.ldr + n0, BN * 4);
+            }
+          }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
@@ -314,6 +444,15 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     if (prev >= 0 && ct == 0) mbar_arrive(&empty[prev]);
     M3R_TR(if (tr && threadIdx.x == 0) tr[5] = gtime_ns();)
 
+    if constexpr (MODE == MODE_PLAIN && (BN == 128 || BN == 256)) {
+      if (p.frag_epi) {
+        uint8_t* stg_frag = smem + STAGES * Cfg::STAGE_BYTES + Cfg::FRAG_STG_OFFSET + wg * 2 * Cfg::FRAG_BUF_BYTES;
+        if (p.out_dtype != 0) epilogue_frag<BN, BF16, true>(p, &tmC, acc, stg_frag, tm * BM + wg * 64, tn * BN, wg, ct);
+        else epilogue_frag<BN, BF16, false>(p, &tmC, acc, stg_frag, tm * BM + wg * 64, tn * BN, wg, ct);
+        M3R_TR(if (tr && threadIdx.x == 0) tr[7] = gtime_ns();)
+        continue;
+      }
+    }
     const int lrow = (tm % tiles_mg) * BM + wg * 64 + r;              // row inside the group
     const int n0 = tn * BN;
     const bool row_ok = lrow < p.M;
@@ -499,6 +638,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     }
     M3R_TR(if (tr && threadIdx.x == 0) tr[7] = gtime_ns();)
   }
+  if constexpr (MODE == MODE_PLAIN) {
+    if (p.frag_epi && ct == 0) bulk_wait_group<0>();   // the shared-memory sources must outlive the stores
+  }
   M3R_TR(if (tr && threadIdx.x == 0) tr[9] = gtime_ns();)
 }
 
@@ -512,6 +654,7 @@ static void fill_params(GemmParams& p, const m3r_gemm_args* a) {
   p.n_peer_out = a->n_peer_out;
   p.trace = trace_buffer();
   p.w_static = a->w_static;
+  p.frag_epi = 0;
   for (int i = 0; i < M3R_MAX_PEERS; ++i) p.peer_out[i] = i < a->n_peer_out ? a->peer_out[i] : nullptr;
   p.groups = 1; p.w_group_rows = 0; p.bias_group = 0;
   p.norm_out = nullptr; p.ldn = 0; p.norm_eps = 0.f; p.stats = nullptr; p.sync = nullptr;
@@ -569,6 +712,15 @@ static int launch_gemm(const m3r_gemm_args* a, cudaStream_t stream, const m3r_ge
       p.ksplit = 2; p.kpart = e->emit_kpart; p.kflag = e->emit_kflag;
     }
   }
+  // A CTA with more than one tile stores through TMA from the fragment-layout epilogue, so that its tensor cores resume
+  // while the stores drain.  One-wave launches, peer stores and the batch row remap keep the transposing epilogue.
+  CUtensorMap tmC;
+  memset(&tmC, 0, sizeof(tmC));
+  if (MODE == MODE_PLAIN && (BN == 128 || BN == 256) && tiles > num_sms() && a->n_peer_out == 0 && a->rows_per_batch <= 0) {
+    const bool f32 = a->out_dtype == M3R_OUT_F32;
+    if (make_tmap_2d(&tmC, a->out, a->is_bf16, (uint64_t)a->N, (uint64_t)a->M, (uint64_t)a->ldc, f32 ? 32 : 64, 64, f32)) return 1;
+    p.frag_epi = 1;
+  }
   const auto kernel = a->is_bf16 ? gemm_kernel<BN, MODE, true> : gemm_kernel<BN, MODE, false>;
   const KernelInfo k = kernel_setup((const void*)kernel, Cfg::SMEM_BYTES_MAX, GEMM_THREADS);
   if (k.resident == 0) return 1;
@@ -583,7 +735,7 @@ static int launch_gemm(const m3r_gemm_args* a, cudaStream_t stream, const m3r_ge
     const int cat = BN >= 256 ? PROF_GEMM256 : (BN >= 128 ? PROF_GEMM128 : PROF_GEMM64);
     ProfScope prof(cat, 2.0 * a->M * groups * (double)a->N * a->K, 2.0 * ((double)a->M * groups * a->K + (double)a->N * groups * a->K) + (double)a->M * groups * a->N * (a->out_dtype ? 2 : 4), stream);
     const size_t smem_bytes = peer_tile ? Cfg::SMEM_BYTES_PEER : Cfg::SMEM_BYTES;
-    cudaError_t le = launch_pdl(kernel, dim3(grid), dim3(GEMM_THREADS), smem_bytes, stream, tmA, tmW, p, tab);
+    cudaError_t le = launch_pdl(kernel, dim3(grid), dim3(GEMM_THREADS), smem_bytes, stream, tmA, tmW, tmC, p, tab);
     if (le != cudaSuccess) return set_error("gemm launch: %s", cudaGetErrorString(le));
   }
   cudaError_t e = cudaGetLastError();

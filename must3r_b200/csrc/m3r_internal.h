@@ -50,10 +50,11 @@ struct ProfScope {
   cudaStream_t stream;
 };
 
-// 2-D TMA descriptor over a row-major 16-bit matrix: inner extent `cols` (contiguous), outer extent `rows`,
-// leading dimension `ld` elements, box = {box_cols, box_rows}, 128-byte swizzle, OOB reads return zeros.
+// 2-D TMA descriptor over a row-major 16-bit (or, with fp32, 32-bit float) matrix: inner extent `cols` (contiguous),
+// outer extent `rows`, leading dimension `ld` elements, box = {box_cols, box_rows}, 128-byte swizzle, OOB reads return
+// zeros and OOB writes are dropped.
 int make_tmap_2d(CUtensorMap* out, const void* base, int is_bf16, uint64_t cols, uint64_t rows, uint64_t ld,
-                 uint32_t box_cols, uint32_t box_rows);
+                 uint32_t box_cols, uint32_t box_rows, bool fp32 = false);
 
 // 3-D variant: {cols, rows, batches}; rows beyond `rows` read as zeros even when the batch stride is larger.
 int make_tmap_3d(CUtensorMap* out, const void* base, int is_bf16, uint64_t cols, uint64_t rows, uint64_t batches,

@@ -93,6 +93,27 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       "r"(c2)
       : "memory");
 }
+// TMA store of a shared-memory box to global memory (rows / columns outside the tensor are not written), tracked as a
+// bulk async-group of the issuing thread.  The writes that filled the box must be made visible to the async proxy first
+// (fence_proxy_async_smem by each writer, then a barrier).
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* smem_src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's bulk groups are still reading their shared-memory source
+template <int N> __device__ __forceinline__ void bulk_wait_group_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+// at most N of this thread's bulk groups are still in flight (their global writes included)
+template <int N> __device__ __forceinline__ void bulk_wait_group() {
+  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
+}
+// brings `bytes` (a multiple of 16, 16-byte aligned) of global memory into L2 without waiting for them
+__device__ __forceinline__ void prefetch_l2_bulk(const void* gptr, uint32_t bytes) {
+  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(reinterpret_cast<uint64_t>(gptr)), "r"(bytes) : "memory");
+}
 
 // ------------------------------------------------------------------ wgmma (sm_90a warpgroup MMA)
 // Shared-memory matrix descriptor for a 128B-swizzled tile whose rows are 128 bytes (64 x 16-bit) and whose 8-row

@@ -103,15 +103,17 @@ static EncodeTiledFn get_encode() {
 }
 
 int make_tmap_2d(CUtensorMap* out, const void* base, int is_bf16, uint64_t cols, uint64_t rows, uint64_t ld,
-                 uint32_t box_cols, uint32_t box_rows) {
+                 uint32_t box_cols, uint32_t box_rows, bool fp32) {
   EncodeTiledFn enc = get_encode();
   if (!enc) return set_error("cuTensorMapEncodeTiled is unavailable (no CUDA driver?)");
   if ((reinterpret_cast<uintptr_t>(base) & 15) != 0) return set_error("TMA base pointer must be 16-byte aligned");
   cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {ld * 2};
+  cuuint64_t strides[1] = {ld * (fp32 ? 4 : 2)};
   cuuint32_t box[2] = {box_cols, box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(out, is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2,
+  const CUtensorMapDataType dt = fp32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                      : (is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
+  CUresult r = enc(out, dt, 2,
                    const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return set_error("cuTensorMapEncodeTiled failed (%d): cols=%llu rows=%llu ld=%llu box=%ux%u",
