@@ -2,8 +2,9 @@
 //
 //   warps 0..7 : two consumer warpgroups -- warpgroup w multiplies rows [64w, 64w + 64) of the 128-row tile with
 //                wgmma.m64nBNk16 (operands straight from the 128B-swizzled smem ring, fp32 accumulator in registers),
-//                then runs the epilogue: bias / RoPE / GELU / residual / image2-embed row bias, vectorised global stores
-//                (a CTA with several tiles: on the accumulator fragment, with TMA stores that drain during the next tile)
+//                then runs the epilogue on the accumulator fragment: bias / RoPE / GELU / residual / image2-embed row
+//                bias in place, then 128-byte column chunks through a swizzled staging buffer to global memory (TMA
+//                stores that drain during the next tile when a CTA owns several tiles, 16-byte thread stores otherwise)
 //   warps 8..11: producer warpgroup -- one elected lane issues TMA (A and W tiles, 128B-swizzled, mbarrier ring); the
 //                warpgroup gives its registers to the consumers (setmaxnreg), whose accumulator is 128 registers at BN = 256
 // The producer keeps filling the ring for the next tile while the consumers drain the current one.  Tiles are walked
@@ -31,24 +32,18 @@ static_assert(128 * GEMM_PRODUCER_REGS + 256 * GEMM_CONSUMER_REGS <= GEMM_LAUNCH
 template <int BN>
 struct GemmCfg {
   static constexpr int STAGE_BYTES = (BM + BN) * BK * 2;
-  static constexpr int STG_BYTES = 2 * 2 * 64 * 33 * 4;        // epilogue transpose: [warpgroup][chunk][64 rows][33]
-  static constexpr int PEER_STAGE_BYTES = 8 * 4096;          // per consumer warp 32 rows x 128 B: transposes peer stores (below)
-  static constexpr int FIXED = 1024 /*align*/ + 256 /*barriers*/ + STG_BYTES;
-  // Only launches that store to peers reserve the peer transpose tile; the others spend that space on the operand ring.
-  static constexpr int STAGES = (SMEM_MAX - FIXED) / STAGE_BYTES;                           // 256:4  192:4  160:5  128:6  64:8  32:9
-  static constexpr int STAGES_PEER = (SMEM_MAX - FIXED - PEER_STAGE_BYTES) / STAGE_BYTES;   // 256:3  192:4  160:4  128:5  64:6  32:8
+  // epilogue staging after the ring: [warpgroup][2 buffers][64 rows x 128 B], 1024-aligned for the 128B swizzle
+  static constexpr int EPI_BUF_BYTES = 64 * 128;
+  static constexpr int FIXED = 1024 /*align*/ + 1024 /*barriers*/ + 2 * 2 * EPI_BUF_BYTES;
+  static constexpr int STAGES = (SMEM_MAX - FIXED) / STAGE_BYTES;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + FIXED;
-  static constexpr int SMEM_BYTES_PEER = STAGES_PEER * STAGE_BYTES + FIXED + PEER_STAGE_BYTES;
-  static constexpr int SMEM_BYTES_MAX = SMEM_BYTES > SMEM_BYTES_PEER ? SMEM_BYTES : SMEM_BYTES_PEER;
-  static_assert(2 * STAGES * 8 <= 256, "ring barriers exceed their space");
-  // the fragment-layout epilogue reuses the transpose area as 1024-aligned TMA store buffers: [warpgroup][2][64 rows x 128 B]
-  static constexpr int FRAG_STG_OFFSET = 1024, FRAG_BUF_BYTES = 64 * 128;
-  static_assert(FRAG_STG_OFFSET + 2 * 2 * FRAG_BUF_BYTES <= 256 + STG_BYTES, "store buffers exceed the epilogue area");
+  static_assert(2 * STAGES * 8 <= 1024, "ring barriers exceed their space");
+  static_assert(STAGES == (BN == 256 ? 4 : BN == 192 ? 4 : BN == 160 ? 5 : BN == 128 ? 6 : BN == 64 ? 8 : 9),
+                "operand ring depth changed");
 };
 
 struct GemmParams {
   int M, N, K;
-  int stages;                  // depth of the operand ring: GemmCfg::STAGES, or STAGES_PEER when the peer tile is reserved
   const float* bias;
   int act;
   const float* residual;
@@ -66,7 +61,7 @@ struct GemmParams {
   void* peer_out[M3R_MAX_PEERS];
   unsigned long long* trace;   // debug only (m3r_debug_trace): 16 words per CTA; normally null
   int w_static;                // weights may be requested before the programmatic-dependency wait
-  int frag_epi;                // epilogue_frag + TMA stores through the output tensor map (persistent plain launches)
+  int tma_store;               // the epilogue stores through TMA and the output tensor map (persistent plain launches)
   // ---- grouped GEMM: `groups` independent problems of M rows each that share the shapes: A rows [g*M, (g+1)*M) of one
   // [groups*M, K] matrix, W rows [g*w_group_rows, +N), bias + g*bias_group, outputs from GemmGroupTab (groups == 1: `out`)
   int groups;
@@ -83,7 +78,7 @@ struct GemmParams {
   // the ks = 1 CTA hands its fp32 accumulator tile to the ks = 0 CTA through `kpart` and a flag, the ks = 0 CTA adds it and
   // runs the epilogue.  Halves the bytes ONE SM pulls from L2, which is what bounds these one-wave GEMMs.
   int ksplit;                  // 1 or 2
-  float4* kpart;               // [tiles][2 column halves][8][128] float4
+  float4* kpart;               // [tiles][BN / 8 accumulator quads][256 consumer threads] float4 (the fragment layout)
   unsigned int* kflag;         // [tiles], zero between launches
 };
 
@@ -95,201 +90,174 @@ struct GemmGroupTab {
 
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f)); }
 
-// Epilogue arithmetic of one 32-column chunk of one accumulator row: bias, RoPE, row bias, GELU, residual -> v[32].
-__device__ __forceinline__ void epilogue_math(const GemmParams& p, const float* bias, const uint32_t (&raw)[32], float (&v)[32], int row,
-                                              bool row_ok, bool rb_on, const float* rope_row, int col0) {
+// The epilogue works on the wgmma accumulator fragment.  Thread (warp w, lane l) of a consumer warpgroup holds rows
+// 16w + l/4 and 16w + l/4 + 8 (h = 0, 1) of the warpgroup's 64, columns 8nb + 2(l%4) + {0, 1} in acc[4nb + 2h + {0, 1}].
+// EpiRows is what the thread needs to know about its two rows (counted inside the group).
+struct EpiRows {
+  bool ok[2], rb_on[2];
+  const float* rope[2];
+  const float* res[2];
+};
+__device__ __forceinline__ EpiRows epi_rows(const GemmParams& p, int lrow) {
+  EpiRows e;
 #pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(raw[i]);
+  for (int h = 0; h < 2; ++h) {
+    const int row = lrow + 8 * h;
+    e.ok[h] = row < p.M;
+    e.rb_on[h] = p.rowbias != nullptr && (row % p.rb_period) >= p.rb_first;
+    e.rope[h] = p.rope_tab ? p.rope_tab + (long long)(row % p.rope_period) * 64 : nullptr;
+    e.res[h] = p.residual ? p.residual + (long long)row * p.ldr : nullptr;
+  }
+  return e;
+}
+
+// Epilogue arithmetic of the 32-column chunk c of the fragment, in place: bias, RoPE, row bias, GELU, residual.  The RoPE
+// partner of column c (c % 32 < 16) is column c + 16, block nb + 2 of the same thread.
+template <int BN>
+__device__ __forceinline__ void epilogue_apply(const GemmParams& p, const EpiRows& rows, const float* bias, float (&acc)[BN / 2],
+                                               int n0, int c, int q) {
+  const int col0 = n0 + 32 * c;
   if (bias) {
 #pragma unroll
-    for (int i = 0; i < 32; i += 4) {
-      const float4 b = __ldg(reinterpret_cast<const float4*>(bias + col0 + i));
-      v[i] += b.x; v[i + 1] += b.y; v[i + 2] += b.z; v[i + 3] += b.w;
+    for (int jj = 0; jj < 4; ++jj) {
+      const int nb = 4 * c + jj;
+      const float2 b = __ldg(reinterpret_cast<const float2*>(bias + n0 + 8 * nb + 2 * q));
+#pragma unroll
+      for (int h = 0; h < 2; ++h) { acc[4 * nb + 2 * h] += b.x; acc[4 * nb + 2 * h + 1] += b.y; }
     }
   }
-  if (rope_row != nullptr && col0 < p.rope_cols && row_ok) {
-    // chunk = half a head: even chunks are the y half (u: 0..15, v: 16..31), odd chunks the x half
-    const float* cs = rope_row + ((col0 >> 5) & 1) * 32;
+  if (p.rope_tab != nullptr && col0 < p.rope_cols) {
 #pragma unroll
-    for (int i = 0; i < 16; i += 4) {
-      const float4 c4 = __ldg(reinterpret_cast<const float4*>(cs + i));
-      const float4 s4 = __ldg(reinterpret_cast<const float4*>(cs + 16 + i));
-      const float cc[4] = {c4.x, c4.y, c4.z, c4.w};
-      const float ss[4] = {s4.x, s4.y, s4.z, s4.w};
+    for (int h = 0; h < 2; ++h) {
+      if (!rows.ok[h]) continue;
+      // chunk = half a head: even chunks are the y half, odd chunks the x half
+      const float* cs = rows.rope[h] + ((col0 >> 5) & 1) * 32;
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float u = v[i + j], w = v[i + j + 16];
-        v[i + j] = u * cc[j] - w * ss[j];
-        v[i + j + 16] = w * cc[j] + u * ss[j];
+      for (int jj = 0; jj < 2; ++jj) {
+        const int i = 8 * jj + 2 * q;
+        const float2 c2 = __ldg(reinterpret_cast<const float2*>(cs + i));
+        const float2 s2 = __ldg(reinterpret_cast<const float2*>(cs + 16 + i));
+        const float cc[2] = {c2.x, c2.y}, ss[2] = {s2.x, s2.y};
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float& vu = acc[4 * (4 * c + jj) + 2 * h + e];
+          float& vw = acc[4 * (4 * c + jj + 2) + 2 * h + e];
+          const float u = vu, w = vw;
+          vu = u * cc[e] - w * ss[e];
+          vw = w * cc[e] + u * ss[e];
+        }
       }
     }
   }
-  if (rb_on) {
 #pragma unroll
-    for (int i = 0; i < 32; i += 4) {
-      const float4 b = __ldg(reinterpret_cast<const float4*>(p.rowbias + col0 + i));
-      v[i] += b.x; v[i + 1] += b.y; v[i + 2] += b.z; v[i + 3] += b.w;
+  for (int h = 0; h < 2; ++h) {
+    if (!rows.rb_on[h]) continue;
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj) {
+      const int nb = 4 * c + jj;
+      const float2 b = __ldg(reinterpret_cast<const float2*>(p.rowbias + n0 + 8 * nb + 2 * q));
+      acc[4 * nb + 2 * h] += b.x; acc[4 * nb + 2 * h + 1] += b.y;
     }
   }
   if (p.act == 1) {
 #pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = gelu_erf(v[i]);
+    for (int i = 16 * c; i < 16 * c + 16; ++i) acc[i] = gelu_erf(acc[i]);
   }
-  if (row_ok && p.residual) {
-    const float4* r4 = reinterpret_cast<const float4*>(p.residual + (long long)row * p.ldr + col0);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const float4 r = r4[i];
-      v[4 * i] += r.x; v[4 * i + 1] += r.y; v[4 * i + 2] += r.z; v[4 * i + 3] += r.w;
-    }
-  }
-}
-
-// Store of one chunk: fp32 or 16-bit row segment; the 16-bit form optionally also goes to the peers' buffers.
-// A peer store instruction of a warp covers 32 rows x 16 B; the four uint4 of a thread complete a 64-byte segment per
-// row back to back, so NVLink sees 64 B write bursts (the fused GEMM -> all-gather path).
-template <bool BF16>
-__device__ __forceinline__ void epilogue_store(const GemmParams& p, void* out, void* const* peers, const float (&v)[32], long long orow, int col0) {
-  if (p.out_dtype == 0) {
-    float4* o4 = reinterpret_cast<float4*>(reinterpret_cast<float*>(out) + orow * p.ldc + col0);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) o4[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-  } else {
-    uint4 w[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      w[i].x = pack16(v[8 * i], v[8 * i + 1], BF16);
-      w[i].y = pack16(v[8 * i + 2], v[8 * i + 3], BF16);
-      w[i].z = pack16(v[8 * i + 4], v[8 * i + 5], BF16);
-      w[i].w = pack16(v[8 * i + 6], v[8 * i + 7], BF16);
-    }
-    uint4* o4 = reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(out) + orow * p.ldc + col0);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) o4[i] = w[i];
-    for (int pr = 0; pr < p.n_peer_out; ++pr) {
-      uint4* q4 = reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(peers[pr]) + orow * p.ldc + col0);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) q4[i] = w[i];
-    }
-  }
-}
-
-// Epilogue of the persistent plain launches, applied to the accumulator fragment in place (no transpose through shared
-// memory).  Thread (warp w, lane l) of a consumer warpgroup holds rows 16w + l/4 and 16w + l/4 + 8 of the warpgroup's 64,
-// columns 8nb + 2(l%4) + {0, 1}; the RoPE partner of column c (c % 32 < 16) is column c + 16, block nb + 2 of the same
-// thread.  The per-element operations and their order are those of epilogue_math (bias, RoPE, row bias, GELU, residual),
-// so the results are bitwise the same.  Each 128-byte-wide column chunk (32 fp32 or 64 16-bit columns) is written into one
-// of the warpgroup's two staging buffers in the 128B-swizzled layout of the output tensor map (the fragment writes are
-// then free of bank conflicts) and leaves with one TMA store that neither the next chunk nor the next tile's MMAs wait for.
-// One barrier per chunk: its elected thread first waits until the previous chunk's store has read the other buffer.
-template <int BN, bool BF16, bool OUT16>
-__device__ __forceinline__ void epilogue_frag(const GemmParams& p, const CUtensorMap* tmC, float (&acc)[BN / 2], uint8_t* stg,
-                                              int row0, int n0, int wg, int ct) {
-  constexpr int CW = OUT16 ? 64 : 32;                // columns per store chunk
-  const int lane = ct & 31, q = lane & 3;
-  const int fr = (ct >> 5) * 16 + (lane >> 2);
-  const int sw = lane >> 2;                          // (row % 8) of both rows: the swizzle phase
-  bool row_ok[2], rb_on[2];
-  const float* rope_row[2];
-  const float* res_row[2];
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int lrow = row0 + fr + 8 * h;
-    row_ok[h] = lrow < p.M;
-    rb_on[h] = p.rowbias != nullptr && (lrow % p.rb_period) >= p.rb_first;
-    rope_row[h] = p.rope_tab ? p.rope_tab + (long long)(lrow % p.rope_period) * 64 : nullptr;
-    res_row[h] = p.residual ? p.residual + (long long)lrow * p.ldr : nullptr;
-  }
-#pragma unroll
-  for (int sc = 0; sc < BN / CW; ++sc) {
-#pragma unroll
-    for (int c = sc * (CW / 32); c < (sc + 1) * (CW / 32); ++c) {
-      const int col0 = n0 + 32 * c;
-      if (p.bias) {
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-          const int nb = 4 * c + jj;
-          const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + 8 * nb + 2 * q));
-#pragma unroll
-          for (int h = 0; h < 2; ++h) { acc[4 * nb + 2 * h] += b.x; acc[4 * nb + 2 * h + 1] += b.y; }
-        }
-      }
-      if (p.rope_tab != nullptr && col0 < p.rope_cols) {
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          if (!row_ok[h]) continue;
-          const float* cs = rope_row[h] + ((col0 >> 5) & 1) * 32;
-#pragma unroll
-          for (int jj = 0; jj < 2; ++jj) {
-            const int i = 8 * jj + 2 * q;
-            const float2 c2 = __ldg(reinterpret_cast<const float2*>(cs + i));
-            const float2 s2 = __ldg(reinterpret_cast<const float2*>(cs + 16 + i));
-            const float cc[2] = {c2.x, c2.y}, ss[2] = {s2.x, s2.y};
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              float& vu = acc[4 * (4 * c + jj) + 2 * h + e];
-              float& vw = acc[4 * (4 * c + jj + 2) + 2 * h + e];
-              const float u = vu, w = vw;
-              vu = u * cc[e] - w * ss[e];
-              vw = w * cc[e] + u * ss[e];
-            }
-          }
-        }
-      }
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        if (!rb_on[h]) continue;
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-          const int nb = 4 * c + jj;
-          const float2 b = __ldg(reinterpret_cast<const float2*>(p.rowbias + n0 + 8 * nb + 2 * q));
-          acc[4 * nb + 2 * h] += b.x; acc[4 * nb + 2 * h + 1] += b.y;
-        }
-      }
-      if (p.act == 1) {
-#pragma unroll
-        for (int i = 16 * c; i < 16 * c + 16; ++i) acc[i] = gelu_erf(acc[i]);
-      }
-      if (p.residual) {
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          if (!row_ok[h]) continue;
-#pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            const int nb = 4 * c + jj;
-            const float2 r = *reinterpret_cast<const float2*>(res_row[h] + n0 + 8 * nb + 2 * q);
-            acc[4 * nb + 2 * h] += r.x; acc[4 * nb + 2 * h + 1] += r.y;
-          }
-        }
-      }
-    }
-    // the chunk's 64 rows x 128 B, row r's 16-byte unit k at r * 128 + ((k ^ (r % 8)) << 4) (SWIZZLE_128B)
-    uint8_t* buf = stg + (sc & 1) * GemmCfg<BN>::FRAG_BUF_BYTES;
+  if (p.residual) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      uint8_t* rowp = buf + (fr + 8 * h) * 128;
-      if constexpr (OUT16) {
+      if (!rows.ok[h]) continue;
 #pragma unroll
-        for (int jj = 0; jj < 8; ++jj) {
-          const int nb = 8 * sc + jj;
-          *reinterpret_cast<uint32_t*>(rowp + ((jj ^ sw) << 4) + 4 * q) = pack16(acc[4 * nb + 2 * h], acc[4 * nb + 2 * h + 1], BF16);
-        }
-      } else {
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-          const int nb = 4 * sc + jj;
-          *reinterpret_cast<float2*>(rowp + (((2 * jj + (q >> 1)) ^ sw) << 4) + 8 * (q & 1)) = make_float2(acc[4 * nb + 2 * h], acc[4 * nb + 2 * h + 1]);
-        }
+      for (int jj = 0; jj < 4; ++jj) {
+        const int nb = 4 * c + jj;
+        const float2 r = *reinterpret_cast<const float2*>(rows.res[h] + n0 + 8 * nb + 2 * q);
+        acc[4 * nb + 2 * h] += r.x; acc[4 * nb + 2 * h + 1] += r.y;
       }
     }
-    fence_proxy_async_smem();
-    if (ct == 0) bulk_wait_group_read<0>();          // the other buffer (next chunk) has been read by its store
-    asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
-    if (ct == 0) {
-      tma_store_2d(tmC, buf, n0 + sc * CW, row0);
-      bulk_commit_group();
+  }
+}
+
+// Writes column chunk sc of the fragment (128 B per row: 32 fp32 or 64 16-bit columns; the last 16-bit chunk of BN 32 and
+// 160 is half as wide) into a 64-row staging buffer, row r's 16-byte unit k at r * 128 + ((k ^ (r % 8)) << 4): the
+// SWIZZLE_128B layout of the output tensor map, in which the fragment writes are free of bank conflicts.
+template <int BN, bool BF16, bool OUT16>
+__device__ __forceinline__ void epilogue_stage(const float (&acc)[BN / 2], uint8_t* buf, int sc, int fr, int q) {
+  const int sw = fr & 7;                             // (row % 8) of both rows: the swizzle phase
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    uint8_t* rowp = buf + (fr + 8 * h) * 128;
+    if constexpr (OUT16) {
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+        const int nb = 8 * sc + jj;
+        if (nb < BN / 8)
+          *reinterpret_cast<uint32_t*>(rowp + ((jj ^ sw) << 4) + 4 * q) = pack16(acc[4 * nb + 2 * h], acc[4 * nb + 2 * h + 1], BF16);
+      }
+    } else {
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const int nb = 4 * sc + jj;
+        *reinterpret_cast<float2*>(rowp + (((2 * jj + (q >> 1)) ^ sw) << 4) + 8 * (q & 1)) = make_float2(acc[4 * nb + 2 * h], acc[4 * nb + 2 * h + 1]);
+      }
     }
   }
+}
+
+// Epilogue of the plain and grouped launches: each chunk is applied, staged in one of the warpgroup's two buffers (they
+// alternate over the CTA's whole sequence of chunks, `nchunk`) and drained after one barrier per chunk.  The barrier of a
+// chunk is passed only after every thread has finished with the chunk before it, so that chunk's buffer is free again.
+// - TMA: one thread stores the chunk with a TMA store that neither the next chunk nor the next tile's MMAs wait for; it
+//   first waits until the previous store has read the other buffer.  Rows past M are clipped by the tensor map.
+// - otherwise every thread copies 16-byte units, 8 consecutive threads per 128-byte row segment, to the output row (after
+//   the rows_per_batch remap; rows past M skipped) and the same unit to every peer's buffer.
+template <int BN, bool BF16, bool OUT16, bool TMA>
+__device__ __forceinline__ void epilogue_out(const GemmParams& p, const CUtensorMap* tmC, const EpiRows& rows, const float* bias,
+                                             float (&acc)[BN / 2], uint8_t* stg, unsigned& nchunk, int lrow0, int n0, int wg, int ct,
+                                             void* out, void* const* peers) {
+  constexpr int CW = OUT16 ? 64 : 32;                // columns per chunk
+  constexpr int NSC = (BN + CW - 1) / CW;
+  const int lane = ct & 31, q = lane & 3;
+  const int fr = (ct >> 5) * 16 + (lane >> 2);
+  // thread copy: rows (ct / 8) + 16 j of the warpgroup's 64, unit ct % 8; byte offset of the unit in chunk 0, -1 past M
+  long long off[4];
+#pragma unroll
+  for (int j = 0; j < 4 && !TMA; ++j) {
+    const int lrow = lrow0 + (ct >> 3) + 16 * j;
+    long long orow = lrow;
+    if (p.rows_per_batch > 0) orow = (long long)(lrow / p.rows_per_batch) * p.batch_stride_rows + lrow % p.rows_per_batch;
+    off[j] = lrow < p.M ? (orow * p.ldc + n0) * (OUT16 ? 2 : 4) + 16 * (ct & 7) : -1;
+  }
+#pragma unroll
+  for (int sc = 0; sc < NSC; ++sc) {
+#pragma unroll
+    for (int c = sc * (CW / 32); c < (sc + 1) * (CW / 32) && c < BN / 32; ++c) epilogue_apply<BN>(p, rows, bias, acc, n0, c, q);
+    // (a TMA launch has an even number of chunks per tile: its buffer follows from sc alone)
+    uint8_t* buf = stg + ((TMA ? sc : nchunk + sc) & 1) * GemmCfg<BN>::EPI_BUF_BYTES;
+    epilogue_stage<BN, BF16, OUT16>(acc, buf, sc, fr, q);
+    if constexpr (TMA) {
+      fence_proxy_async_smem();
+      if (ct == 0) bulk_wait_group_read<0>();
+    }
+    asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+    if constexpr (TMA) {
+      if (ct == 0) {
+        tma_store_2d(tmC, buf, n0 + sc * CW, lrow0);
+        bulk_commit_group();
+      }
+      continue;
+    }
+    if ((sc + 1) * CW > BN && (ct & 7) >= 4) continue;     // half chunk: 64 B per row
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      if (off[j] < 0) continue;
+      const int rr = (ct >> 3) + 16 * j;
+      const uint4 val = *reinterpret_cast<const uint4*>(buf + rr * 128 + (((ct & 7) ^ (rr & 7)) << 4));
+      const long long o = off[j] + sc * 128;
+      *reinterpret_cast<uint4*>(reinterpret_cast<uint8_t*>(out) + o) = val;
+      for (int pr = 0; pr < p.n_peer_out; ++pr) *reinterpret_cast<uint4*>(reinterpret_cast<uint8_t*>(peers[pr]) + o) = val;
+    }
+  }
+  nchunk += NSC;
 }
 
 __device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int* p) {
@@ -313,7 +281,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
             const __grid_constant__ CUtensorMap tmC, const GemmParams p, const __grid_constant__ typename TabOf<MODE>::type tab) {
   using Cfg = GemmCfg<BN>;
-  const int STAGES = p.stages;
+  constexpr int STAGES = Cfg::STAGES;
   constexpr int NCHUNK = BN / 32;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -322,7 +290,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
   uint64_t* full = bars;                  // [STAGES]
   uint64_t* empty = bars + STAGES;        // [STAGES]
-  float* stg_all = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES + 256);    // [2 warpgroups][2 chunks][64][33]
+  uint8_t* epi_stg = smem + STAGES * Cfg::STAGE_BYTES + 1024;     // [2 warpgroups][2][64 rows x 128 B] epilogue staging
 
   M3R_TR(unsigned long long* tr = p.trace ? p.trace + 16ull * blockIdx.x : nullptr;
          if (tr && threadIdx.x == 0) { tr[0] = gtime_ns(); tr[8] = smid(); })
@@ -387,7 +355,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           }
           if constexpr (MODE == MODE_PLAIN) {
             // the tile's residual rows, spread over its k-blocks, go to L2 ahead of the epilogue's fragment-layout loads
-            if (p.frag_epi && p.residual) {
+            if (p.tma_store && p.residual) {
               for (int r = kb; r < BM; r += num_kb)
                 if (m0 + r < p.M) prefetch_l2_bulk(p.residual + (long long)(m0 + r) * p.ldr + n0, BN * 4);
             }
@@ -410,9 +378,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   const int wg = warp >> 2;                       // rows [64 wg, 64 wg + 64) of the tile
   const int ct = threadIdx.x & 127;
   const int wl = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
-  const int u = ct >> 6;                          // epilogue: which chunk of a pair this thread drains ...
-  const int r = ct & 63;                          // ... for which row of the warpgroup's 64
-  float* stg = stg_all + wg * (2 * 64 * 33);
+  const int fr = wl * 16 + (lane >> 2), q = lane & 3;   // the thread's fragment rows fr, fr + 8 and column pair 2q (epi_rows)
+  uint8_t* stg = epi_stg + wg * 2 * Cfg::EPI_BUF_BYTES;
+  unsigned nchunk = 0;                            // chunks staged so far: selects the staging buffer
   int stage = 0; uint32_t phase = 0;
   for (int t = tile0; t < num_tiles; t += tile_step) {
     const int tm = t % tiles_m, tn = t / tiles_m;
@@ -444,66 +412,17 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     if (prev >= 0 && ct == 0) mbar_arrive(&empty[prev]);
     M3R_TR(if (tr && threadIdx.x == 0) tr[5] = gtime_ns();)
 
-    if constexpr (MODE == MODE_PLAIN && (BN == 128 || BN == 256)) {
-      if (p.frag_epi) {
-        uint8_t* stg_frag = smem + STAGES * Cfg::STAGE_BYTES + Cfg::FRAG_STG_OFFSET + wg * 2 * Cfg::FRAG_BUF_BYTES;
-        if (p.out_dtype != 0) epilogue_frag<BN, BF16, true>(p, &tmC, acc, stg_frag, tm * BM + wg * 64, tn * BN, wg, ct);
-        else epilogue_frag<BN, BF16, false>(p, &tmC, acc, stg_frag, tm * BM + wg * 64, tn * BN, wg, ct);
-        M3R_TR(if (tr && threadIdx.x == 0) tr[7] = gtime_ns();)
-        continue;
-      }
-    }
-    const int lrow = (tm % tiles_mg) * BM + wg * 64 + r;              // row inside the group
+    const int lrow0 = (tm % tiles_mg) * BM + wg * 64;                 // the warpgroup's first row, counted inside the group
     const int n0 = tn * BN;
-    const bool row_ok = lrow < p.M;
-    long long orow = lrow;
-    if (p.rows_per_batch > 0) orow = (long long)(lrow / p.rows_per_batch) * p.batch_stride_rows + lrow % p.rows_per_batch;
-    const bool rb_on = p.rowbias != nullptr && (lrow % p.rb_period) >= p.rb_first;
-    const float* rope_row = p.rope_tab ? p.rope_tab + (long long)(lrow % p.rope_period) * 64 : nullptr;
     const float* bias = p.bias ? p.bias + (long long)g * p.bias_group : nullptr;
-    void* out_g = p.out;
-    void* const* peers_g = p.peer_out;
-    if constexpr (MODE == MODE_GROUPED) { out_g = tab.out[g]; peers_g = tab.peer[g]; }
-
-    // The accumulator fragments are transposed through shared memory two 32-column chunks at a time, so that each
-    // epilogue thread owns 32 consecutive columns of ONE row (the layout the bias / RoPE / LayerNorm code works on):
-    // chunks c and c + 1 of the warpgroup's 64 rows go to smem, thread (u, r) reads back row r of chunk c + u.
-    auto stage_pair = [&](int c, uint32_t (&raw)[32]) {
-      asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");        // the previous pair has been read
-#pragma unroll
-      for (int uu = 0; uu < 2; ++uu) {
-        if (c + uu < NCHUNK) {
-#pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            const int nb = (c + uu) * 4 + jj;
-            float* s0 = stg + uu * (64 * 33) + (wl * 16 + (lane >> 2)) * 33 + jj * 8 + 2 * (lane & 3);
-            s0[0] = acc[nb * 4]; s0[1] = acc[nb * 4 + 1];
-            s0[8 * 33] = acc[nb * 4 + 2]; s0[8 * 33 + 1] = acc[nb * 4 + 3];
-          }
-        }
-      }
-      asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
-      if (c + u < NCHUNK) {
-        const float* s1 = stg + u * (64 * 33) + r * 33;
-#pragma unroll
-        for (int i = 0; i < 32; ++i) raw[i] = __float_as_uint(s1[i]);
-      }
-    };
     if constexpr (MODE == MODE_EMIT) {
-      // ---- x = acc + bias + residual -> out (fp32); the thread keeps its values (chunks u, u + 2, ...) for the normalisation
-      constexpr int CPT = BN / 64;                                 // 32-column chunks per thread
-      uint32_t rawc[CPT][32];
-#pragma unroll
-      for (int pi = 0; pi < CPT; ++pi) stage_pair(2 * pi, rawc[pi]);
-      const int rit = wg * 64 + r;                                 // row in tile
-      if (ksplit > 1) {                                            // BN == 64 only (host)
-        // [tile][column chunk][8 float4][128 rows]: lanes are consecutive rows -> 512 B per warp request
-        uint32_t (&raw)[32] = rawc[0];
-        float4* kp = p.kpart + ((long long)(t * NCHUNK + u) * 8) * BM + rit;
+      // ---- LayerNorm-emitting epilogue (one tile per CTA).  Split-K: the ks = 1 CTA hands its raw accumulator over in the
+      // fragment layout ([tile][acc / 4][256 threads]: lanes are consecutive float4, 512 B per warp request) and is done.
+      if (ksplit > 1) {
+        float4* kp = p.kpart + (long long)t * (BN / 8) * 256 + threadIdx.x;
         if (ks == 1) {
 #pragma unroll
-          for (int i = 0; i < 8; ++i)
-            kp[(long long)i * BM] = make_float4(__uint_as_float(raw[4 * i]), __uint_as_float(raw[4 * i + 1]), __uint_as_float(raw[4 * i + 2]), __uint_as_float(raw[4 * i + 3]));
+          for (int i = 0; i < BN / 8; ++i) kp[i * 256] = make_float4(acc[4 * i], acc[4 * i + 1], acc[4 * i + 2], acc[4 * i + 3]);
           __threadfence();
           asm volatile("bar.sync 1, 256;" ::: "memory");
           if (threadIdx.x == 0) atom_add_release_u32(p.kflag + t, 1u);
@@ -516,19 +435,43 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         }
         asm volatile("bar.sync 1, 256;" ::: "memory");
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float4 o = __ldcg(kp + (long long)i * BM);
-          raw[4 * i] = __float_as_uint(__uint_as_float(raw[4 * i]) + o.x); raw[4 * i + 1] = __float_as_uint(__uint_as_float(raw[4 * i + 1]) + o.y);
-          raw[4 * i + 2] = __float_as_uint(__uint_as_float(raw[4 * i + 2]) + o.z); raw[4 * i + 3] = __float_as_uint(__uint_as_float(raw[4 * i + 3]) + o.w);
+        for (int i = 0; i < BN / 8; ++i) {
+          const float4 o = __ldcg(kp + i * 256);
+          acc[4 * i] += o.x; acc[4 * i + 1] += o.y; acc[4 * i + 2] += o.z; acc[4 * i + 3] += o.w;
+        }
+      }
+      // x = acc + bias + residual -> out (fp32).  Chunks c and c + 1 are applied and staged (fp32) together; thread (u, r)
+      // reads back row r of chunk c + u and keeps it (chunks u, u + 2, ...) for the normalisation.
+      constexpr int CPT = BN / 64;                                 // 32-column chunks per thread
+      const int u = ct >> 6, r = ct & 63;
+      const int lrow = lrow0 + r;
+      const bool row_ok = lrow < p.M;
+      long long orow = lrow;
+      if (p.rows_per_batch > 0) orow = (long long)(lrow / p.rows_per_batch) * p.batch_stride_rows + lrow % p.rows_per_batch;
+      const int rit = wg * 64 + r;                                 // row in tile
+      const EpiRows rows = epi_rows(p, lrow0 + fr);
+      float v[CPT][32];
+#pragma unroll
+      for (int pi = 0; pi < CPT; ++pi) {
+        if (pi > 0) asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");     // the previous pair has been read
+#pragma unroll
+        for (int uu = 0; uu < 2; ++uu) {
+          epilogue_apply<BN>(p, rows, bias, acc, n0, 2 * pi + uu, q);
+          epilogue_stage<BN, BF16, false>(acc, stg + uu * Cfg::EPI_BUF_BYTES, 2 * pi + uu, fr, q);
+        }
+        asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+        const uint8_t* rowp = stg + u * Cfg::EPI_BUF_BYTES + r * 128;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+          const float4 x = *reinterpret_cast<const float4*>(rowp + ((k ^ (r & 7)) << 4));
+          v[pi][4 * k] = x.x; v[pi][4 * k + 1] = x.y; v[pi][4 * k + 2] = x.z; v[pi][4 * k + 3] = x.w;
         }
       }
       const int parts = NCHUNK * tiles_n;                          // 32-column partials per row
       float2* st = p.stats + ((long long)tm * parts) * BM;
-      float v[CPT][32];
 #pragma unroll
       for (int pi = 0; pi < CPT; ++pi) {
         const int cc = 2 * pi + u;
-        epilogue_math(p, bias, rawc[pi], v[pi], lrow, row_ok, rb_on, rope_row, n0 + cc * 32);
         if (!row_ok) {
 #pragma unroll
           for (int i = 0; i < 32; ++i) v[pi][i] = 0.f;
@@ -552,7 +495,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       // sit in front of the fence above)
       if (row_ok) {
 #pragma unroll
-        for (int pi = 0; pi < CPT; ++pi) epilogue_store<BF16>(p, p.out, p.peer_out, v[pi], orow, n0 + (2 * pi + u) * 32);
+        for (int pi = 0; pi < CPT; ++pi) {
+          float4* o4 = reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + orow * p.ldc + n0 + (2 * pi + u) * 32);
+#pragma unroll
+          for (int i = 0; i < 8; ++i) o4[i] = make_float4(v[pi][4 * i], v[pi][4 * i + 1], v[pi][4 * i + 2], v[pi][4 * i + 3]);
+        }
       }
       if (threadIdx.x == 0) {
         unsigned int spins = 0;
@@ -591,55 +538,21 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       }
       continue;
     }
-#pragma unroll
-    for (int c = 0; c < NCHUNK; c += 2) {
-      uint32_t raw[32];
-      stage_pair(c, raw);
-      const int cc = c + u;                                              // this thread's chunk
-      if (p.n_peer_out > 0 && p.out_dtype != 0) {
-        // ---- fused GEMM -> all-gather epilogue.  A thread owns one ROW of the chunk, so direct peer stores would be 32
-        // scattered 16-byte pieces per instruction - partial sectors over NVLink.  The warp's 32 rows x 32 columns go
-        // through a swizzled shared-memory tile and leave as 64-byte row segments: one store instruction = 8 rows x 64 B
-        // (4 lanes per row), whole sectors, to every peer's buffer.  (u and cc are uniform across a warp.)
-        if (cc < NCHUNK) {
-          uint4* pst = reinterpret_cast<uint4*>(stg_all + 2 * (2 * 64 * 33)) + warp * 256;      // [32 rows][8 x 16 B]
-          const int row_base = (tm % tiles_mg) * BM + wg * 64 + (r & ~31);
-          float v[32];
-          epilogue_math(p, bias, raw, v, lrow, row_ok, rb_on, rope_row, n0 + cc * 32);
-          uint4* o4 = reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(out_g) + orow * p.ldc + n0 + cc * 32);
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            uint4 w;
-            w.x = pack16(v[8 * i], v[8 * i + 1], BF16); w.y = pack16(v[8 * i + 2], v[8 * i + 3], BF16);
-            w.z = pack16(v[8 * i + 4], v[8 * i + 5], BF16); w.w = pack16(v[8 * i + 6], v[8 * i + 7], BF16);
-            if (row_ok) o4[i] = w;                                  // this GPU's copy: the thread's own row
-            pst[lane * 8 + (i ^ (lane & 7))] = w;
-          }
-          __syncwarp();
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const int rr = k * 8 + lane / 4, piece = lane % 4;
-            const int row_r = row_base + rr;
-            if (row_r < p.M) {
-              long long orow_r = row_r;
-              if (p.rows_per_batch > 0) orow_r = (long long)(row_r / p.rows_per_batch) * p.batch_stride_rows + row_r % p.rows_per_batch;
-              const uint4 val = pst[rr * 8 + (piece ^ (rr & 7))];
-              for (int pr = 0; pr < p.n_peer_out; ++pr)
-                reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(peers_g[pr]) + orow_r * p.ldc + n0 + cc * 32)[piece] = val;
-            }
-          }
-          __syncwarp();
-        }
-      } else if (cc < NCHUNK) {
-        float v[32];
-        epilogue_math(p, bias, raw, v, lrow, row_ok, rb_on, rope_row, n0 + cc * 32);
-        if (row_ok) epilogue_store<BF16>(p, out_g, peers_g, v, orow, n0 + cc * 32);
-      }
+    void* out_g = p.out;
+    void* const* peers_g = p.peer_out;
+    if constexpr (MODE == MODE_GROUPED) { out_g = tab.out[g]; peers_g = tab.peer[g]; }
+    const EpiRows rows = epi_rows(p, lrow0 + fr);
+    if (MODE == MODE_PLAIN && (BN == 128 || BN == 256) && p.tma_store) {
+      if (p.out_dtype != 0) epilogue_out<BN, BF16, true, true>(p, &tmC, rows, bias, acc, stg, nchunk, lrow0, n0, wg, ct, out_g, peers_g);
+      else epilogue_out<BN, BF16, false, true>(p, &tmC, rows, bias, acc, stg, nchunk, lrow0, n0, wg, ct, out_g, peers_g);
+    } else {
+      if (p.out_dtype != 0) epilogue_out<BN, BF16, true, false>(p, &tmC, rows, bias, acc, stg, nchunk, lrow0, n0, wg, ct, out_g, peers_g);
+      else epilogue_out<BN, BF16, false, false>(p, &tmC, rows, bias, acc, stg, nchunk, lrow0, n0, wg, ct, out_g, peers_g);
     }
     M3R_TR(if (tr && threadIdx.x == 0) tr[7] = gtime_ns();)
   }
   if constexpr (MODE == MODE_PLAIN) {
-    if (p.frag_epi && ct == 0) bulk_wait_group<0>();   // the shared-memory sources must outlive the stores
+    if (p.tma_store && ct == 0) bulk_wait_group<0>();   // the shared-memory sources must outlive the stores
   }
   M3R_TR(if (tr && threadIdx.x == 0) tr[9] = gtime_ns();)
 }
@@ -654,7 +567,7 @@ static void fill_params(GemmParams& p, const m3r_gemm_args* a) {
   p.n_peer_out = a->n_peer_out;
   p.trace = trace_buffer();
   p.w_static = a->w_static;
-  p.frag_epi = 0;
+  p.tma_store = 0;
   for (int i = 0; i < M3R_MAX_PEERS; ++i) p.peer_out[i] = i < a->n_peer_out ? a->peer_out[i] : nullptr;
   p.groups = 1; p.w_group_rows = 0; p.bias_group = 0;
   p.norm_out = nullptr; p.ldn = 0; p.norm_eps = 0.f; p.stats = nullptr; p.sync = nullptr;
@@ -712,21 +625,19 @@ static int launch_gemm(const m3r_gemm_args* a, cudaStream_t stream, const m3r_ge
       p.ksplit = 2; p.kpart = e->emit_kpart; p.kflag = e->emit_kflag;
     }
   }
-  // A CTA with more than one tile stores through TMA from the fragment-layout epilogue, so that its tensor cores resume
-  // while the stores drain.  One-wave launches, peer stores and the batch row remap keep the transposing epilogue.
+  // A CTA with more than one tile stores through TMA, so that its tensor cores resume while the stores drain.  One-wave
+  // launches, peer stores and the batch row remap store from the threads.
   CUtensorMap tmC;
   memset(&tmC, 0, sizeof(tmC));
   if (MODE == MODE_PLAIN && (BN == 128 || BN == 256) && tiles > num_sms() && a->n_peer_out == 0 && a->rows_per_batch <= 0) {
     const bool f32 = a->out_dtype == M3R_OUT_F32;
     if (make_tmap_2d(&tmC, a->out, a->is_bf16, (uint64_t)a->N, (uint64_t)a->M, (uint64_t)a->ldc, f32 ? 32 : 64, 64, f32)) return 1;
-    p.frag_epi = 1;
+    p.tma_store = 1;
   }
   const auto kernel = a->is_bf16 ? gemm_kernel<BN, MODE, true> : gemm_kernel<BN, MODE, false>;
-  const KernelInfo k = kernel_setup((const void*)kernel, Cfg::SMEM_BYTES_MAX, GEMM_THREADS);
+  const KernelInfo k = kernel_setup((const void*)kernel, Cfg::SMEM_BYTES, GEMM_THREADS);
   if (k.resident == 0) return 1;
   if (k.regs < GEMM_LAUNCH_REGS) return set_error("gemm: kernel built with %d registers per thread, the register split needs %d", k.regs, GEMM_LAUNCH_REGS);
-  const bool peer_tile = a->n_peer_out > 0 && a->out_dtype != 0;
-  p.stages = peer_tile ? Cfg::STAGES_PEER : Cfg::STAGES;
   int grid = tiles < num_sms() ? tiles : num_sms();
   if (MODE == MODE_EMIT) grid = tiles * p.ksplit;
   if (MODE == MODE_GROUPED && grp->max_ctas > 0 && grid > grp->max_ctas) grid = grp->max_ctas;
@@ -734,8 +645,7 @@ static int launch_gemm(const m3r_gemm_args* a, cudaStream_t stream, const m3r_ge
   {
     const int cat = BN >= 256 ? PROF_GEMM256 : (BN >= 128 ? PROF_GEMM128 : PROF_GEMM64);
     ProfScope prof(cat, 2.0 * a->M * groups * (double)a->N * a->K, 2.0 * ((double)a->M * groups * a->K + (double)a->N * groups * a->K) + (double)a->M * groups * a->N * (a->out_dtype ? 2 : 4), stream);
-    const size_t smem_bytes = peer_tile ? Cfg::SMEM_BYTES_PEER : Cfg::SMEM_BYTES;
-    cudaError_t le = launch_pdl(kernel, dim3(grid), dim3(GEMM_THREADS), smem_bytes, stream, tmA, tmW, tmC, p, tab);
+    cudaError_t le = launch_pdl(kernel, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, tmA, tmW, tmC, p, tab);
     if (le != cudaSuccess) return set_error("gemm launch: %s", cudaGetErrorString(le));
   }
   cudaError_t e = cudaGetLastError();

@@ -1,11 +1,11 @@
-"""The epilogue of persistent plain GEMM launches (more tiles than SMs, so every CTA owns several tiles): it works on the
-accumulator fragment and writes through TMA stores that drain while the next tile's MMAs run.
+"""The epilogue of persistent plain GEMM launches (more tiles than SMs, so every CTA owns several tiles) drains its
+staged chunks through TMA stores that complete while the next tile's MMAs run.
 
 Each epilogue form is checked three ways, at BN 256 and 128, fp16 and bf16, with M a multiple of the tile height and M
 ragged:
 - against fp32 torch math on the same 16-bit inputs;
-- bitwise against the first rows computed by a one-wave launch (few enough tiles for one per CTA), which takes the
-  transposing epilogue: both epilogues must apply the same operations in the same order;
+- bitwise against the first rows computed by a one-wave launch (few enough tiles for one per CTA), whose threads copy
+  the staged chunks to global memory: both drains must store the same values;
 - output memory outside the [M, N] result (rows past M, columns beside a column slice) must stay untouched, so a store
   that is dropped or lands in the wrong place fails."""
 import os
