@@ -237,6 +237,41 @@ int m3r_pointgrid_query(const float* queries, const int32_t* qbucket, int32_t Q,
                         const int64_t* cell_keys, const int32_t* cell_off, int32_t C, const int32_t* bucket_cells,
                         int32_t nb, float h, float inv_h, float* out, void* stream);
 
+/* One frame's camera and keyframe test in the SLAM front end (must3r/slam/model.py:147-172 get_camera_pose, :62-91
+ * get_overlap_score, :231-235 the keyframe decision): a small device record per view, read back once by the host. */
+typedef struct {
+  float c2w[16];          /* camera-to-world, row-major 4x4 */
+  float w2c[16];          /* its rigid inverse */
+  float focal;            /* Weiszfeld focal in pixels, clamped below at 0 */
+  float conf_mean;        /* mean of conf */
+  float conf_median;      /* lower median of conf (torch.median); NaN if any conf is NaN */
+  int32_t n_conf;         /* subsampled points with conf > min_conf_keyframe (m3r_slam_keyframe) */
+  double score;           /* overlap score (m3r_slam_keyframe) */
+  int32_t keyframe;       /* keyframe decision (m3r_slam_keyframe) */
+  int32_t reserved;
+} m3r_slam_record;
+/* overlap modes of m3r_slam_keyframe */
+#define M3R_OVERLAP_NN 0
+#define M3R_OVERLAP_NN_NORM 1
+#define M3R_OVERLAP_MEANCONF 2
+#define M3R_OVERLAP_MEDIANCONF 3
+/* B views of [H, W]: pts3d [B,H,W,3], pts3d_local [B,H,W,3], conf [B,H,W] fp32 -> rec[B].  focal = the Weiszfeld fit of
+ * pixel - (ppx, ppy) ~ focal * (x, y) / z (closed-form L2 start, 10 re-weighted steps).  Unless is_first: when
+ * has_seq_focal, pts3d_local's z is scaled IN PLACE by seq_focal / focal (fp32, as the reference); then the rotation and
+ * translation minimising sum (conf - 1) |R x_local + t - x_world|^2 (Horn's quaternion, det R = +1).  is_first gives
+ * the identity pose.  Each view is one thread-block cluster; one launch. */
+int m3r_slam_pose(const float* pts3d, float* pts3d_local, const float* conf, int32_t B, int32_t H, int32_t W, float ppx,
+                  float ppy, int32_t has_seq_focal, float seq_focal, int32_t is_first, m3r_slam_record* rec, void* stream);
+/* Overlap score and keyframe decision of one view whose record m3r_slam_pose wrote.  The subsampled points are the
+ * pixels (s*i, s*j) of [H, W] (s = subsamp); dists [ceil(H/s) * ceil(W/s)] = the nearest-map-point distance of every
+ * one of them, conf [H,W] and pts3d_local [H,W,3] the full maps.  NN modes: the `percentile` (np.percentile, linear)
+ * of dists (divided by z + 1e-9 for NN_NORM) over the points with conf > min_conf_keyframe, +inf counted as FLT_MAX,
+ * NaN if one of them is NaN, 0 if there is none; the conf modes take the record's mean / median.  keyframe = is_first
+ * or ((score > thr for NN modes, score < thr otherwise) and conf_median > min_conf_keyframe). */
+int m3r_slam_keyframe(const float* dists, const float* conf, const float* pts3d_local, int32_t H, int32_t W, int32_t subsamp,
+                      int32_t mode, double percentile, double thr, float min_conf_keyframe, int32_t is_first,
+                      m3r_slam_record* rec, void* stream);
+
 /* ---------------------------------------------------------------------------------------------------
  * Input preprocessing of V RGB uint8 frames of one size: src [V, src_h, src_w, 3] uint8 (HWC; pixel stride 3 bytes,
  * row pitch src_pitch bytes, frame stride src_vstride bytes - a crop view or a padded frame needs no copy) -> fp32

@@ -9,6 +9,7 @@ from __future__ import annotations
 import ctypes as C
 from typing import Optional
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -340,3 +341,66 @@ def postprocess_raw(pm: torch.Tensor):
     conf = torch.empty(pm.shape[:-1], device=pm.device, dtype=torch.float32)
     _lib.check(_lib.lib().m3r_postprocess(_p(pm), P, _p(pts), _p(loc), _p(conf), _stream()), "postprocess")
     return pts, loc, conf
+
+
+# m3r_slam_record (include/must3r_b200.h): one view's camera and keyframe test, as a host numpy record
+SLAM_RECORD = np.dtype([("c2w", "<f4", (4, 4)), ("w2c", "<f4", (4, 4)), ("focal", "<f4"), ("conf_mean", "<f4"),
+                        ("conf_median", "<f4"), ("n_conf", "<i4"), ("score", "<f8"), ("keyframe", "<i4"),
+                        ("reserved", "<i4")])
+
+
+def overlap_mode_id(mode: str) -> int:
+    """must3r/slam/model.py:72-90: 'meanconf', 'medianconf', or any mode containing 'nn' ('norm' divides by the depth)."""
+    if mode == "meanconf":
+        return 2
+    if mode == "medianconf":
+        return 3
+    if "nn" in mode:
+        return 1 if "norm" in mode else 0
+    raise ValueError(f"Unknown overlap score method {mode}")
+
+
+def slam_record_c2w(rec: torch.Tensor) -> torch.Tensor:
+    """Device view [B,4,4] fp32 of the c2w field of records [B, SLAM_RECORD.itemsize] uint8."""
+    return rec[:, :64].view(torch.float32).view(-1, 4, 4)
+
+
+def slam_pose(pts3d: torch.Tensor, pts3d_local: torch.Tensor, conf: torch.Tensor, seq_focal: Optional[float] = None,
+              is_first: bool = False, rec: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Focal, pose and confidence statistics of B views (csrc/slam.cu): pts3d, pts3d_local [B,H,W,3], conf [B,H,W] fp32
+    contiguous.  Unless is_first, pts3d_local's z is scaled in place by seq_focal / focal when seq_focal is given.
+    Returns the records [B, SLAM_RECORD.itemsize] uint8 on the device (or fills `rec`)."""
+    _req_cuda(pts3d, pts3d_local, conf)
+    for t in (pts3d, pts3d_local, conf):
+        assert t.dtype == torch.float32 and t.is_contiguous()
+    B, H, W = conf.shape
+    assert pts3d.shape == (B, H, W, 3) and pts3d_local.shape == (B, H, W, 3)
+    if rec is None:
+        rec = torch.empty((B, SLAM_RECORD.itemsize), dtype=torch.uint8, device=conf.device)
+    assert rec.shape == (B, SLAM_RECORD.itemsize) and rec.is_contiguous()
+    _lib.check(_lib.lib().m3r_slam_pose(_p(pts3d), _p(pts3d_local), _p(conf), B, H, W, W / 2, H / 2,
+                                        int(seq_focal is not None), 0.0 if seq_focal is None else float(seq_focal),
+                                        int(bool(is_first)), _p(rec), _stream()), "slam_pose")
+    return rec
+
+
+def slam_keyframe(dists: Optional[torch.Tensor], conf: torch.Tensor, pts3d_local: torch.Tensor, rec: torch.Tensor, *,
+                  subsamp: Optional[int], mode: str, percentile: float, thr: float, min_conf_keyframe: float,
+                  is_first: bool) -> torch.Tensor:
+    """Overlap score and keyframe decision of one view into its record rec [1, SLAM_RECORD.itemsize] (csrc/slam.cu).
+    conf [H,W], pts3d_local [H,W,3] fp32 contiguous; dists = the distances of every subsampled pixel (::subsamp in both
+    axes, row-major; None for the conf modes)."""
+    _req_cuda(dists, conf, pts3d_local, rec)
+    H, W = conf.shape
+    s = int(subsamp) if subsamp else 1
+    m = overlap_mode_id(mode)
+    assert conf.dtype == torch.float32 and conf.is_contiguous()
+    assert pts3d_local.dtype == torch.float32 and pts3d_local.is_contiguous() and pts3d_local.shape == (H, W, 3)
+    if m <= 1:
+        assert dists is not None and dists.dtype == torch.float32 and dists.is_contiguous()
+        assert dists.numel() == ((H + s - 1) // s) * ((W + s - 1) // s)
+    assert rec.shape[-1] == SLAM_RECORD.itemsize and rec.is_contiguous()
+    _lib.check(_lib.lib().m3r_slam_keyframe(_p(dists) if m <= 1 else None, _p(conf), _p(pts3d_local), H, W, s, m,
+                                            float(percentile), float(thr), float(min_conf_keyframe), int(bool(is_first)),
+                                            _p(rec), _stream()), "slam_keyframe")
+    return rec

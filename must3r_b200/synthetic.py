@@ -114,3 +114,16 @@ def rel_l2(a: torch.Tensor, b: torch.Tensor) -> float:
     a = a.detach().double().cpu()
     b = b.detach().double().cpu()
     return float((a - b).norm() / b.norm().clamp_min(1e-30))
+
+
+def camera_like_head_bias(dsd: Dict[str, torch.Tensor], gain: float = 0.5, depth: float = 2.0) -> Dict[str, torch.Tensor]:
+    """Shift the decoder head's bias (in place) so that a random network predicts camera-like point maps: points in front
+    of the camera (z > 0) whose x and y grow with the pixel's column and row inside each 16x16 patch (world and local
+    channels alike).  The SLAM front end's Weiszfeld focal is then positive, as with a trained model."""
+    i, j = torch.meshgrid(torch.arange(16.0), torch.arange(16.0), indexing="ij")
+    bias = dsd["head_dec.proj.bias"].view(-1, 256)
+    for c0 in (0, 3):
+        bias[c0] += gain * ((j - 7.5) / 8).flatten()
+        bias[c0 + 1] += gain * ((i - 7.5) / 8).flatten()
+        bias[c0 + 2] += depth
+    return dsd
