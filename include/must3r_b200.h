@@ -272,6 +272,30 @@ int m3r_slam_keyframe(const float* dists, const float* conf, const float* pts3d_
                       int32_t mode, double percentile, double thr, float min_conf_keyframe, int32_t is_first,
                       m3r_slam_record* rec, void* stream);
 
+/* Confidence-filtered point cloud of a reconstructed scene at T thresholds (must3r/demo/gradio.py:131-156
+ * get_3D_model_from_scene with as_pointcloud, :91-92 the masking).  A device table of V views, each of its own H x W: */
+typedef struct {
+  const float* pts3d;     /* [H,W,3]: world points, or local points when c2w is set */
+  const float* c2w;       /* NULL, or the 4x4 row-major camera-to-world applied to pts3d (geotrf, local_pointmaps) */
+  const float* conf;      /* [H,W] */
+  const float* img;       /* [3,H,W] ImgNorm image; colour = clip(x * 0.5 + 0.5, 0, 1) (dust3r rgb) */
+  int32_t H, W;
+  int64_t first_tile;     /* sum over the earlier views of ceil(H * W / M3R_SCENE_TILE) */
+} m3r_scene_view;
+#define M3R_SCENE_TILE 1024
+#define M3R_SCENE_MAX_THR 8
+/* Pass 1: tile_counts [T, n_tiles] int32 = pixels of each tile with conf >= thr[t] (thr: T fp32 on the device; NaN conf
+ * is never selected), tile_off [T, n_tiles] int64 = their exclusive prefix in tile order, counts [T] int64 = the totals.
+ * n_tiles = the first_tile the view after the last one would have. */
+int m3r_scene_count(const m3r_scene_view* views, int32_t V, const float* thr, int32_t T, int64_t n_tiles,
+                    int32_t* tile_counts, int64_t* tile_off, int64_t* counts, void* stream);
+/* Pass 2, one launch for every view and threshold: the points of threshold t go to rows [base_t, base_t + counts[t]) of
+ * pts_out / col_out [sum(counts), 3] fp32, base_t = counts[0] + ... + counts[t-1], view-major then in raster order (the
+ * order of numpy's boolean masking); nothing else is written.  tile_off and counts come from m3r_scene_count on the same
+ * views and thresholds. */
+int m3r_scene_points(const m3r_scene_view* views, int32_t V, const float* thr, int32_t T, int64_t n_tiles,
+                     const int64_t* tile_off, const int64_t* counts, float* pts_out, float* col_out, void* stream);
+
 /* ---------------------------------------------------------------------------------------------------
  * Input preprocessing of V RGB uint8 frames of one size: src [V, src_h, src_w, 3] uint8 (HWC; pixel stride 3 bytes,
  * row pitch src_pitch bytes, frame stride src_vstride bytes - a crop view or a padded frame needs no copy) -> fp32

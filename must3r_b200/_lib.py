@@ -91,6 +91,10 @@ SIGNATURES = {
                                 C.c_int32, C.c_float, C.c_int32, C.c_void_p, C.c_void_p]),
     "m3r_slam_keyframe": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double,
                                     C.c_double, C.c_float, C.c_int32, C.c_void_p, C.c_void_p]),
+    "m3r_scene_count": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p,
+                                  C.c_void_p, C.c_void_p]),
+    "m3r_scene_points": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p,
+                                   C.c_void_p, C.c_void_p, C.c_void_p]),
     "m3r_resample_pil_u8": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32,
                                       C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                       C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,

@@ -384,6 +384,71 @@ def slam_pose(pts3d: torch.Tensor, pts3d_local: torch.Tensor, conf: torch.Tensor
     return rec
 
 
+SCENE_VIEW = np.dtype([("pts3d", "<u8"), ("c2w", "<u8"), ("conf", "<u8"), ("img", "<u8"), ("H", "<i4"), ("W", "<i4"),
+                       ("first_tile", "<i8")])           # m3r_scene_view
+SCENE_TILE = 1024
+SCENE_MAX_THR = 8
+
+
+def scene_points(pts3d, conf, imgs, thresholds, c2w=None, out=None):
+    """Point clouds of V views at T <= 8 confidence thresholds in one pass over the views (csrc/scene.cu).
+
+    pts3d: V fp32 [H,W,3] (world points; local points when c2w, V fp32 [4,4] camera-to-world, is given), conf: V fp32
+    [H,W], imgs: V fp32 [3,H,W] ImgNorm images, all contiguous CUDA tensors; views may differ in H x W.  Threshold t
+    keeps the pixels with conf >= thresholds[t] (never a NaN conf), view after view in raster order.
+    Returns (pts [N,3], col [N,3], counts): N = sum(counts), threshold t's points are rows sum(counts[:t]) onwards, col
+    is clip(img * 0.5 + 0.5, 0, 1).  counts (host ints) are read back once to size the outputs.  out = (pts, col) fp32
+    CUDA buffers of at least N rows receives the points instead; rows past N are not written."""
+    V = len(conf)
+    T = len(thresholds)
+    if V < 1 or len(pts3d) != V or len(imgs) != V or (c2w is not None and len(c2w) != V):
+        raise ValueError(f"scene_points: {len(pts3d)} pointmaps, {V} confidence maps, {len(imgs)} images")
+    if not 1 <= T <= SCENE_MAX_THR:
+        raise ValueError(f"scene_points: {T} thresholds (1..{SCENE_MAX_THR})")
+    dev = conf[0].device
+    table = np.zeros(V, dtype=SCENE_VIEW)
+    first = 0
+    for v in range(V):
+        p, c, im = pts3d[v], conf[v], imgs[v]
+        m = None if c2w is None else c2w[v]
+        _req_cuda(p, c, im, m)
+        H, W = c.shape
+        for t, shape in ((p, (H, W, 3)), (c, (H, W)), (im, (3, H, W))) + (() if m is None else ((m, (4, 4)),)):
+            if t.dtype != torch.float32 or not t.is_contiguous() or tuple(t.shape) != shape or t.device != dev:
+                raise ValueError(f"scene_points: view {v}: expected contiguous fp32 {shape} on {dev}, got "
+                                 f"{t.dtype} {tuple(t.shape)} on {t.device}")
+        if H * W == 0:
+            raise ValueError(f"scene_points: view {v} is empty")
+        table[v] = (p.data_ptr(), 0 if m is None else m.data_ptr(), c.data_ptr(), im.data_ptr(), H, W, first)
+        first += (H * W + SCENE_TILE - 1) // SCENE_TILE
+    n_tiles = first
+    views = torch.from_numpy(table.view(np.uint8)).pin_memory().to(dev, non_blocking=True)
+    thr = torch.tensor([float(t) for t in thresholds], dtype=torch.float32).pin_memory().to(dev, non_blocking=True)
+    tile_counts = torch.empty((T, n_tiles), dtype=torch.int32, device=dev)
+    tile_off = torch.empty((T, n_tiles), dtype=torch.int64, device=dev)
+    counts = torch.empty((T,), dtype=torch.int64, device=dev)
+    _lib.check(_lib.lib().m3r_scene_count(_p(views), V, _p(thr), T, n_tiles, _p(tile_counts), _p(tile_off), _p(counts),
+                                          _stream()), "scene_count")
+    host = torch.empty((T,), dtype=torch.int64, pin_memory=True)
+    host.copy_(counts, non_blocking=True)
+    torch.cuda.current_stream(dev).synchronize()
+    n = [int(v) for v in host.tolist()]
+    total = sum(n)
+    if out is None:
+        pts = torch.empty((total, 3), dtype=torch.float32, device=dev)
+        col = torch.empty((total, 3), dtype=torch.float32, device=dev)
+    else:
+        pts, col = out
+        _req_cuda(pts, col)
+        for b in (pts, col):
+            if b.dtype != torch.float32 or not b.is_contiguous() or b.dim() != 2 or b.shape[1] != 3 or b.shape[0] < total:
+                raise ValueError(f"scene_points: out buffers must be contiguous fp32 [>= {total}, 3]")
+    if total:
+        _lib.check(_lib.lib().m3r_scene_points(_p(views), V, _p(thr), T, n_tiles, _p(tile_off), _p(counts), _p(pts), _p(col),
+                                               _stream()), "scene_points")
+    return pts[:total], col[:total], n
+
+
 def slam_keyframe(dists: Optional[torch.Tensor], conf: torch.Tensor, pts3d_local: torch.Tensor, rec: torch.Tensor, *,
                   subsamp: Optional[int], mode: str, percentile: float, thr: float, min_conf_keyframe: float,
                   is_first: bool) -> torch.Tensor:
