@@ -95,7 +95,9 @@ typedef struct {
    * A operand of the next GEMM, whose weight / bias carry the LayerNorm affine (W * diag(gamma), b + W beta).  The CTAs
    * holding the column tiles of one 128-row block exchange per-row (mean, M2) partials through device memory and meet
    * at a device-scope counter, so the whole problem must fit in one wave (ceil(M/128) * N/64 <= SM count) and such
-   * launches must not run concurrently on two streams of one device. */
+   * launches must not run concurrently on two streams of one device.  norm_out rows are not remapped, so norm_out
+   * cannot be combined with rows_per_batch > 0 (an argument error).
+   * Base pointers: bias, rowbias, rope_tab and residual 8-byte aligned; out, peer_out and norm_out 16-byte aligned. */
   void* norm_out;
   int64_t ldn;
   float norm_eps;

@@ -330,12 +330,18 @@ static int grid_for(long long total, int block) {
 
 using namespace m3r;
 
+// The row kernels move float4 (fp32) and uint2 (16-bit) units: base pointers off that grid are refused before any launch.
+static bool misaligned(const void* ptr, unsigned bytes) { return ptr && (reinterpret_cast<uintptr_t>(ptr) % bytes) != 0; }
+
 static int layernorm_impl(const float* x, int64_t ldx, const float* add, int64_t ldadd, int add_rows, int add_period, const float* gamma,
                           const float* beta, float eps, int32_t M, int32_t D, void* out, int64_t ldo,
                           int32_t out_dtype, int32_t is_bf16, void* stream) {
   if (!x || !out) return set_error("layernorm: null pointer");
   if (M <= 0) return 0;
   if (D % 4 || D > 2048 || ldx % 4 || (add && ldadd % 4) || ldo % 4) return set_error("layernorm: D=%d must be a multiple of 4, <= 2048, 16B-aligned rows", D);
+  if (misaligned(x, 16) || misaligned(add, 16) || misaligned(gamma, 16) || misaligned(beta, 16))
+    return set_error("layernorm: x, add, gamma and beta must be 16-byte aligned (float4 loads)");
+  if (misaligned(out, out_dtype == M3R_OUT_F32 ? 16 : 8)) return set_error("layernorm: out must be %d-byte aligned", out_dtype == M3R_OUT_F32 ? 16 : 8);
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   const int wpb = M <= 4096 ? 4 : 8;          // small row counts: more, smaller blocks cover more SMs
   const int grid = (M + wpb - 1) / wpb;
@@ -367,6 +373,8 @@ extern "C" int m3r_layernorm16(const void* x16, int64_t ldx, const float* gamma,
   if (!x16 || !gamma || !beta || !out16) return set_error("layernorm16: null pointer");
   if (M <= 0) return 0;
   if (D % 4 || D > 2048 || ldx % 4 || ldo % 4) return set_error("layernorm16: D=%d must be a multiple of 4, <= 2048, 8B-aligned rows", D);
+  if (misaligned(x16, 8) || misaligned(out16, 8)) return set_error("layernorm16: x16 and out16 must be 8-byte aligned");
+  if (misaligned(gamma, 16) || misaligned(beta, 16)) return set_error("layernorm16: gamma and beta must be 16-byte aligned");
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   const int wpb = M <= 4096 ? 4 : 8;
   const int grid = (M + wpb - 1) / wpb;
@@ -384,6 +392,8 @@ static int cast16_impl(const float* x, int64_t ldx, const float* add, int64_t ld
   if (!x || !out) return set_error("cast16: null pointer");
   if (M <= 0) return 0;
   if (D % 4 || ldx % 4 || ldo % 4 || (add && ldadd % 4)) return set_error("cast16: alignment");
+  if (misaligned(x, 16) || misaligned(add, 16)) return set_error("cast16: x and add must be 16-byte aligned (float4 loads)");
+  if (misaligned(out, 8)) return set_error("cast16: out must be 8-byte aligned");
   launch_pdl(cast16_kernel, dim3(grid_for((long long)M * (D / 4), 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),
              x, (long long)ldx, add, (long long)ldadd, (int)M, (int)D, reinterpret_cast<uint16_t*>(out), (long long)ldo, (int)is_bf16);
   return check_launch("cast16");

@@ -654,6 +654,10 @@ static int launch_gemm(const m3r_gemm_args* a, cudaStream_t stream, const m3r_ge
   return 0;
 }
 
+static bool misaligned(const void* ptr, unsigned bytes) { return ptr && (reinterpret_cast<uintptr_t>(ptr) % bytes) != 0; }
+
+// The epilogue reads bias / rowbias / rope_tab / residual as float2 and stores out / peers / norm_out in 16-byte units;
+// a base pointer off that grid would fault on the device, so it is refused here, before any CUDA call.
 static int check_args(const m3r_gemm_args* a) {
   if (!a || !a->A || !a->W) return set_error("gemm: null pointer");
   if (a->N % 32 || a->K % 64 || a->N <= 0 || a->K <= 0) return set_error("gemm: N (%d) must be a multiple of 32 and K (%d) of 64", a->N, a->K);
@@ -662,6 +666,10 @@ static int check_args(const m3r_gemm_args* a) {
   if (a->residual && a->ldr % 4) return set_error("gemm: ldr alignment");
   if (a->rope_tab && (a->rope_cols % 64)) return set_error("gemm: rope_cols must be a multiple of 64");
   if (a->n_peer_out < 0 || a->n_peer_out > M3R_MAX_PEERS || (a->n_peer_out > 0 && a->out_dtype != M3R_OUT_16)) return set_error("gemm: peer outputs need 0..%d pointers and a 16-bit output", M3R_MAX_PEERS);
+  if (misaligned(a->bias, 8)) return set_error("gemm: bias must be 8-byte aligned");
+  if (misaligned(a->rowbias, 8)) return set_error("gemm: rowbias must be 8-byte aligned");
+  if (misaligned(a->rope_tab, 8)) return set_error("gemm: rope_tab must be 8-byte aligned");
+  if (misaligned(a->residual, 8)) return set_error("gemm: residual must be 8-byte aligned");
   return 0;
 }
 
@@ -687,6 +695,11 @@ extern "C" int m3r_gemm(const m3r_gemm_args* a, void* stream) {
   using namespace m3r;
   if (check_args(a)) return 1;
   if (!a->out) return set_error("gemm: null pointer");
+  if (misaligned(a->out, 16)) return set_error("gemm: out must be 16-byte aligned");
+  for (int r = 0; r < a->n_peer_out; ++r)
+    if (!a->peer_out[r] || misaligned(a->peer_out[r], 16)) return set_error("gemm: peer_out[%d] must be a 16-byte aligned pointer", r);
+  if (a->norm_out && misaligned(a->norm_out, 16)) return set_error("gemm: norm_out must be 16-byte aligned");
+  if (a->norm_out && a->rows_per_batch > 0) return set_error("gemm: norm_out does not take the rows_per_batch remap");
   if (a->M <= 0) return 0;
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   const int sms = num_sms();
@@ -722,7 +735,15 @@ extern "C" int m3r_gemm_grouped(const m3r_gemm_args* a, const m3r_gemm_group* gr
   if (check_args(a)) return 1;
   if (!grp || grp->groups < 1 || grp->groups > M3R_MAX_GROUPS) return set_error("gemm_grouped: 1..%d groups", M3R_MAX_GROUPS);
   if (a->norm_out || a->residual) return set_error("gemm_grouped: no residual / norm_out");
-  for (int g = 0; g < grp->groups; ++g) if (!grp->out[g]) return set_error("gemm_grouped: out[%d] is null", g);
+  if (a->bias && grp->bias_group % 2) return set_error("gemm_grouped: bias_group must keep every group's bias 8-byte aligned");
+  for (int g = 0; g < grp->groups; ++g) {
+    if (!grp->out[g]) return set_error("gemm_grouped: out[%d] is null", g);
+    if (misaligned(grp->out[g], 16)) return set_error("gemm_grouped: out[%d] must be 16-byte aligned", g);
+    for (int r = 0; r < a->n_peer_out; ++r) {
+      const void* pr = grp->peer_out[g * M3R_MAX_PEERS + r];
+      if (!pr || misaligned(pr, 16)) return set_error("gemm_grouped: peer_out[%d] must be a 16-byte aligned pointer", g * M3R_MAX_PEERS + r);
+    }
+  }
   if (a->M <= 0) return 0;
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   int bn = pick_bn(a->M, a->N, grp->groups);

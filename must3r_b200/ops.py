@@ -82,9 +82,12 @@ def linear(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None
     return out
 
 
-def linear_grouped(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], outs, *, peer_ptrs=None) -> None:
+def linear_grouped(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], outs, *, peer_ptrs=None,
+                   rows_per_batch: int = 0, batch_stride_rows: int = 0, max_ctas: int = 0) -> None:
     """`groups` GEMMs of one shape in a single launch: a [G, M, K], w [G, N, K] (any row stride between groups),
-    bias [G, N] or None, outs = list of G 16-bit tensors [M, N] (one common row stride)."""
+    bias [G, N] or None, outs = list of G 16-bit tensors [M, N] (one common row stride).
+    rows_per_batch > 0: row r of every group goes to output row (r // rows_per_batch) * batch_stride_rows +
+    r % rows_per_batch (the memory append into [B, cap, N] buffers).  max_ctas > 0: run on at most that many SMs."""
     _req_cuda(a, w)
     G, M, K = a.shape
     N = w.shape[1]
@@ -94,8 +97,9 @@ def linear_grouped(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor
     args.M, args.N, args.K, args.is_bf16 = M, N, K, F16[a.dtype]
     args.bias = bias.data_ptr() if bias is not None else None
     args.ldc, args.out_dtype = outs[0].stride(0), 0 if outs[0].dtype == torch.float32 else 1
+    args.rows_per_batch, args.batch_stride_rows = rows_per_batch, batch_stride_rows
     grp = _lib.GemmGroup()
-    grp.groups, grp.w_group_rows = G, w.stride(0) // K
+    grp.groups, grp.w_group_rows, grp.max_ctas = G, w.stride(0) // K, max_ctas
     grp.bias_group = bias.stride(0) if bias is not None else 0
     for g in range(G):
         assert outs[g].stride(0) == outs[0].stride(0) and outs[g].stride(1) == 1
