@@ -160,7 +160,8 @@ int m3r_add_cast16(const float* x, int64_t ldx, const float* add, int64_t ldadd,
 int m3r_rope_table(const int64_t* pos, int32_t T, float base, float f0, float* tab, void* stream);
 
 /* Stand-alone in-place 2-D RoPE with the curope operator contract (curope.cpp:49-69):
- * tokens [B,N,H,D=64] 16-bit or fp32 with strides (sB,sN,sH,1) in elements, pos [B,N,2] int64. */
+ * tokens [B,N,H,D=64] 16-bit or fp32 with strides (sB,sN,sH,1) in elements, pos [B,N,2] int64.
+ * B, N, H and D must not be negative (an argument error, even when their product is positive); D % 4 == 0. */
 int m3r_rope_2d(void* tokens, int32_t dtype /*0 f32,1 f16,2 bf16*/, int32_t B, int32_t N, int32_t H, int32_t D,
                 int64_t sB, int64_t sN, int64_t sH, const int64_t* pos, float base, float fwd, void* stream);
 
@@ -200,7 +201,9 @@ int m3r_attention(const m3r_attn_args* args, void* stream);
 /* Merge `n` exported attention states of the same queries over disjoint key sets:
  * out[r, c] = sum_k o_k[r, c] 2^(m_k[r,h] - m) / sum_k l_k[r,h] 2^(m_k[r,h] - m), m = max_k m_k, h = c / 64.
  * parts_o[k] / parts_ml[k]: device pointers as exported above (rows x H*64 fp32, rows x H x 2 fp32); out: [rows, H*64]
- * 16-bit with leading dim ldo.  m3r_attn_state_fill writes the state of an EMPTY key set (o = 0, m = -inf, l = 0). */
+ * 16-bit with leading dim ldo.  m3r_attn_state_fill writes the state of an EMPTY key set (o = 0, m = -inf, l = 0).
+ * Base pointers: every parts_o[k], out and export_o 16-byte aligned and every parts_ml[k] and export_ml 8-byte aligned
+ * (non-null parts), refused before any CUDA call otherwise. */
 int m3r_attn_merge(const float* const* parts_o, const float* const* parts_ml, int32_t n, int64_t rows, int32_t H,
                    void* out, int64_t ldo, int32_t is_bf16, void* stream);
 int m3r_attn_state_fill(float* export_o, float* export_ml, int64_t rows, int32_t H, void* stream);
@@ -209,11 +212,12 @@ int m3r_attn_state_fill(float* export_o, float* export_ml, int64_t rows, int32_t
  * Patch embedding front end: im2col of [V,3,H,W] fp32 images into [V*N, 768] 16-bit rows
  * (col = c*256 + i*16 + j, the flattened Conv2d(3,D,16,16) weight order, dust3r/croco/models/blocks.py:222),
  * to be followed by m3r_gemm with the [D,768] weight.  Tokens in raster order (patch_embed.py:20-29).
+ * Base pointers: img 16-byte aligned (float4 loads), out 8-byte aligned; refused before any CUDA call otherwise.
  * ------------------------------------------------------------------------------------------------- */
 int m3r_im2col16(const float* img, int32_t V, int32_t H, int32_t W, void* out, int32_t is_bf16, void* stream);
 
 /* Head unpatchify (must3r/tools/image.py:9-14 + head.py:71): proj [V*N,1792] fp32 ->
- * out[v,16y+i,16x+j,c] = proj[v, y*w+x, c*256+16i+j], out [V,H,W,7] fp32. */
+ * out[v,16y+i,16x+j,c] = proj[v, y*w+x, c*256+16i+j], out [V,H,W,7] fp32.  C (7 for the model) must be >= 1. */
 int m3r_unpatchify(const float* proj, int32_t V, int32_t H, int32_t W, int32_t C, float* out, void* stream);
 
 /* postprocess(compute_cam=False) (must3r/engine/inference.py:16-27, must3r/tools/geometry.py:14-18):
@@ -458,7 +462,8 @@ int m3r_ipc_close(void* ptr);
  * m3r_peer_wait(local_flags = this rank's own array, rank_mask, value): a kernel that spins on the GPU until every slot r
  * with bit r of rank_mask set has reached `value`; work enqueued after it sees the rows those ranks stored. */
 /* Copy `bytes` (multiple of 16) from src to the same-sized block dsts[k], k < n: this GPU's staging buffer and its peers'
- * (NVLink stores): the exchange step of the context-parallel cross-attention. */
+ * (NVLink stores): the exchange step of the context-parallel cross-attention.  src and every dsts[k] must be non-null and
+ * 16-byte aligned (uint4 loads and stores), refused before any CUDA call otherwise. */
 int m3r_peer_bcast(const void* src, void* const* dsts, int32_t n, int64_t bytes, void* stream);
 int m3r_peer_signal(void* const* flag_slots, int32_t n, uint32_t value, void* stream);
 int m3r_peer_wait(const void* local_flags, uint32_t rank_mask, uint32_t value, void* stream);

@@ -420,6 +420,7 @@ extern "C" int m3r_rope_table(const int64_t* pos, int32_t T, float base, float f
 extern "C" int m3r_rope_2d(void* tokens, int32_t dtype, int32_t B, int32_t N, int32_t H, int32_t D, int64_t sB,
                            int64_t sN, int64_t sH, const int64_t* pos, float base, float fwd, void* stream) {
   if (!tokens || !pos) return set_error("rope_2d: null pointer");
+  if (B < 0 || N < 0 || H < 0 || D < 0) return set_error("rope_2d: negative dimension (B=%d, N=%d, H=%d, D=%d)", B, N, H, D);
   if (D % 4) return set_error("rope_2d: token dim must be multiple of 4");   // kernels.cu:94
   const long long total = (long long)B * N * H * (D / 2);
   if (total <= 0) return 0;
@@ -436,6 +437,8 @@ extern "C" int m3r_rope_2d(void* tokens, int32_t dtype, int32_t B, int32_t N, in
 extern "C" int m3r_im2col16(const float* img, int32_t V, int32_t H, int32_t W, void* out, int32_t is_bf16, void* stream) {
   if (!img || !out) return set_error("im2col16: null pointer");
   if (H % 16 || W % 16) return set_error("im2col16: image size (%d,%d) is not a multiple of the patch size 16", H, W);
+  if (misaligned(img, 16)) return set_error("im2col16: img must be 16-byte aligned (float4 loads)");
+  if (misaligned(out, 8)) return set_error("im2col16: out must be 8-byte aligned");
   if (V <= 0) return 0;
   launch_pdl(im2col16_kernel, dim3(grid_for((long long)V * 3 * H * (W / 4), 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),
              img, (int)V, (int)H, (int)W, reinterpret_cast<uint16_t*>(out), (int)is_bf16);
@@ -445,6 +448,7 @@ extern "C" int m3r_im2col16(const float* img, int32_t V, int32_t H, int32_t W, v
 extern "C" int m3r_unpatchify(const float* proj, int32_t V, int32_t H, int32_t W, int32_t C, float* out, void* stream) {
   if (!proj || !out) return set_error("unpatchify: null pointer");
   if (H % 16 || W % 16) return set_error("unpatchify: bad image size");
+  if (C < 1) return set_error("unpatchify: C=%d channels, must be >= 1", C);
   if (V <= 0) return 0;
   launch_pdl(unpatchify_kernel, dim3(grid_for((long long)V * H * W, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), proj, (int)V, (int)H, (int)W, (int)C, out);
   return check_launch("unpatchify");
@@ -462,6 +466,11 @@ extern "C" int m3r_attn_merge(const float* const* parts_o, const float* const* p
   if (!parts_o || !parts_ml || !out || n < 1 || n > M3R_MAX_PEERS) return set_error("attn_merge: 1..%d states", M3R_MAX_PEERS);
   if (rows <= 0) return 0;
   if (ldo % 8) return set_error("attn_merge: ldo must be a multiple of 8");
+  for (int k = 0; k < n; ++k) {
+    if (!parts_o[k] || misaligned(parts_o[k], 16)) return set_error("attn_merge: parts_o[%d] must be a 16-byte aligned pointer", k);
+    if (!parts_ml[k] || misaligned(parts_ml[k], 8)) return set_error("attn_merge: parts_ml[%d] must be an 8-byte aligned pointer", k);
+  }
+  if (misaligned(out, 16)) return set_error("attn_merge: out must be 16-byte aligned");
   PartList pl;
   for (int k = 0; k < M3R_MAX_PEERS; ++k) { pl.o[k] = k < n ? parts_o[k] : nullptr; pl.ml[k] = k < n ? reinterpret_cast<const float2*>(parts_ml[k]) : nullptr; }
   launch_pdl(attn_merge_kernel, dim3(grid_for(rows * H * 8, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), pl, (int)n,
@@ -471,6 +480,8 @@ extern "C" int m3r_attn_merge(const float* const* parts_o, const float* const* p
 
 extern "C" int m3r_attn_state_fill(float* export_o, float* export_ml, int64_t rows, int32_t H, void* stream) {
   if (!export_o || !export_ml) return set_error("attn_state_fill: null pointer");
+  if (misaligned(export_o, 16)) return set_error("attn_state_fill: export_o must be 16-byte aligned (float4 stores)");
+  if (misaligned(export_ml, 8)) return set_error("attn_state_fill: export_ml must be 8-byte aligned (float2 stores)");
   if (rows <= 0) return 0;
   launch_pdl(attn_state_fill_kernel, dim3(grid_for(rows * H * 16, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),
              reinterpret_cast<float4*>(export_o), (long long)(rows * H * 16), reinterpret_cast<float2*>(export_ml), (long long)(rows * H));
@@ -479,6 +490,9 @@ extern "C" int m3r_attn_state_fill(float* export_o, float* export_ml, int64_t ro
 
 extern "C" int m3r_peer_bcast(const void* src, void* const* dsts, int32_t n, int64_t bytes, void* stream) {
   if (!src || !dsts || n < 1 || n > M3R_MAX_PEERS || bytes % 16) return set_error("peer_bcast: 1..%d destinations, bytes %% 16 == 0", M3R_MAX_PEERS);
+  if (misaligned(src, 16)) return set_error("peer_bcast: src must be 16-byte aligned (uint4 loads)");
+  for (int k = 0; k < n; ++k)
+    if (!dsts[k] || misaligned(dsts[k], 16)) return set_error("peer_bcast: dsts[%d] must be a non-null, 16-byte aligned pointer", k);
   if (bytes <= 0) return 0;
   DstList dl;
   for (int k = 0; k < M3R_MAX_PEERS; ++k) dl.p[k] = k < n ? reinterpret_cast<uint4*>(dsts[k]) : nullptr;

@@ -185,6 +185,10 @@ def rope_2d(tokens: torch.Tensor, positions: torch.Tensor, base: float, fwd: flo
         raise RuntimeError("seq_length differs between tokens & positions")
     if positions.size(2) != 2:
         raise RuntimeError("positions.shape[2] must be equal to 2")
+    if positions.device != tokens.device:
+        raise RuntimeError("tokens and positions are not on the same device")
+    if positions.dtype != torch.int64:                    # curope reads them through data_ptr<int64_t>(), which throws
+        raise RuntimeError(f"expected scalar type Long but found {positions.dtype} (positions must be int64)")
     _req_cuda(tokens, positions)
     if tokens.stride(3) != 1:
         raise RuntimeError("tokens are not contiguous")

@@ -22,7 +22,8 @@ Epilogue, fp32 round-to-nearest, in the kernel's order (epilogue_apply), x the v
 error bound; every rounding is at most U |result| and |result| <= |ref| + E:
   bias, row bias, residual add   E' = E + U (|x'| + E)
   RoPE (u' = u cos - w sin)      E' = |cos| E_u + |sin| E_w + U ((|u| + E_u)|cos| + (|w| + E_w)|sin|) + U (|u'| + ...)
-                                 (two products and one add, or an fma; the fp32 table values are exact inputs)
+                                 (two products and one add, or an fma; the fp32 table values are exact inputs, or
+                                 with rope_tab_err the exact trig plus |u| e_cos + |w| e_sin, elementwise_ref.py)
   GELU 0.5 x (1 + erf(x/sqrt2))  E' = 1.13 E                              |gelu'| <= 1.129
                                     + 0.5 (|x| + E) U (4 |erf| + 2.26 |z| + |1 + erf|) + U |y|
                                  4 U |erf|: erff within 2 ulp; 2.26 U |z|: z = x * fl(1/sqrt2) is within 2U |z| of
@@ -101,10 +102,14 @@ def _add(v, e, t):
     return v, e + U32 * (v.abs() + e)
 
 
-def rope_apply(v, e, tab, rows, rope_cols, rope_period):
+def rope_apply(v, e, tab, rows, rope_cols, rope_period, tab_err=None):
     """RoPE of columns < rope_cols in 64-wide heads (32-column chunks: even = y half, odd = x half of the table) on the
-    float64 value v and its bound e; tab [>= rope_period, 64] fp32, rows = the group-local row indices."""
+    float64 value v and its bound e; tab [>= rope_period, 64] fp32, rows = the group-local row indices.  tab_err (same
+    shape as tab): the table is the exact float64 trig and the kernel's fp32 table errs by at most tab_err per entry,
+    which adds (|u| + E_u) e_cos + (|w| + E_w) e_sin before the fp32 terms (whose |cos|, |sin| grow by e_cos, e_sin).
+    Without it the fp32 table values are exact inputs, as the docstring above states."""
     t = tab[rows % rope_period].double()
+    te = tab_err[rows % rope_period].double() if tab_err is not None else None
     v, e = v.clone(), e.clone()
     for c0 in range(0, rope_cols, 32):
         h = (c0 // 32) % 2
@@ -113,8 +118,16 @@ def rope_apply(v, e, tab, rows, rope_cols, rope_period):
         eu, ew = e[:, c0:c0 + 16].clone(), e[:, c0 + 16:c0 + 32].clone()
         ca, sa = cs.abs(), sn.abs()
         nu, nw = uu * cs - ww * sn, ww * cs + uu * sn
-        base_u = ca * eu + sa * ew + U32 * ((uu.abs() + eu) * ca + (ww.abs() + ew) * sa)
-        base_w = ca * ew + sa * eu + U32 * ((ww.abs() + ew) * ca + (uu.abs() + eu) * sa)
+        if te is not None:
+            ec, es = te[:, 32 * h:32 * h + 16], te[:, 32 * h + 16:32 * h + 32]
+            tu = (uu.abs() + eu) * ec + (ww.abs() + ew) * es
+            tw = (ww.abs() + ew) * ec + (uu.abs() + eu) * es
+            ca, sa = ca + ec, sa + es
+            base_u = tu + ca * eu + sa * ew + U32 * ((uu.abs() + eu) * ca + (ww.abs() + ew) * sa)
+            base_w = tw + ca * ew + sa * eu + U32 * ((ww.abs() + ew) * ca + (uu.abs() + eu) * sa)
+        else:
+            base_u = ca * eu + sa * ew + U32 * ((uu.abs() + eu) * ca + (ww.abs() + ew) * sa)
+            base_w = ca * ew + sa * eu + U32 * ((ww.abs() + ew) * ca + (uu.abs() + eu) * sa)
         v[:, c0:c0 + 16], v[:, c0 + 16:c0 + 32] = nu, nw
         e[:, c0:c0 + 16] = base_u + U32 * (nu.abs() + base_u)
         e[:, c0 + 16:c0 + 32] = base_w + U32 * (nw.abs() + base_w)
@@ -130,9 +143,11 @@ def gelu_apply(v, e):
 
 
 def reference(a, w, *, M, N, K, groups=1, w_group_rows=0, bias=None, bias_group=0, act=0, residual=None,
-              rowbias=None, rb_period=1, rb_first=0, rope_tab=None, rope_cols=0, rope_period=1, ksplit=1) -> Ref:
+              rowbias=None, rb_period=1, rb_first=0, rope_tab=None, rope_cols=0, rope_period=1, ksplit=1,
+              rope_tab_err=None) -> Ref:
     """a: [groups * M, >= K] 16-bit (group g = rows [g M, (g + 1) M)); w: [>= (groups - 1) w_group_rows + N, >= K];
-    bias: 1-D fp32 (group g at g * bias_group); residual: [M, >= N] fp32; rope_tab: [>= rope_period, 64] fp32."""
+    bias: 1-D fp32 (group g at g * bias_group); residual: [M, >= N] fp32; rope_tab: [>= rope_period, 64] fp32, or the
+    exact float64 table with rope_tab_err the bound of the kernel table's error (rope_apply)."""
     dev = a.device
     f64 = dict(dtype=torch.float64, device=dev)
     val = torch.empty(groups * M, N, **f64)
@@ -150,7 +165,7 @@ def reference(a, w, *, M, N, K, groups=1, w_group_rows=0, bias=None, bias_group=
             if bg is not None:
                 v, e = _add(v, e, bg)
             if rope_tab is not None and rope_cols > 0:
-                v, e = rope_apply(v, e, rope_tab, rows, rope_cols, rope_period)
+                v, e = rope_apply(v, e, rope_tab, rows, rope_cols, rope_period, rope_tab_err)
             if rowbias is not None:
                 on = ((rows % rb_period) >= rb_first)[:, None]
                 v2, e2 = _add(v, e, rowbias[:N].double())
@@ -219,7 +234,7 @@ def check(out, val, bnd, what="", M=None, bn=None) -> float:
     allowance, naming its group, row, column, tile (at tile width bn) and 32-column chunk; return the worst
     err / allowance."""
     err = (out.double() - val).abs()
-    ratio = err / bnd
+    ratio = torch.where(err == 0, torch.zeros_like(err), err / bnd)      # an exact result passes a zero allowance
     bad = ~(ratio <= 1)                                                   # also catches NaN
     if bool(bad.any()):
         i = int(bad.flatten().nonzero()[0])

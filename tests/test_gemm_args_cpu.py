@@ -1,6 +1,8 @@
-"""Base pointers the GEMM epilogue and the LayerNorm / cast kernels would access off their vector width are refused
-with a message that names the argument, before any CUDA call: the library is called through ctypes with made-up
-device addresses that are misaligned by 4 or 8 bytes, so no device is touched (and none is needed)."""
+"""Base pointers the GEMM epilogue, the LayerNorm / cast kernels, im2col16, the attention state merge / fill and the peer
+broadcast would access off their vector width are refused with a message that names the argument, before any CUDA call:
+the library is called through ctypes with made-up device addresses that are misaligned by 2, 4 or 8 bytes, so no device
+is touched (and none is needed).  So are a null broadcast destination, negative RoPE dimensions and an unpatchify
+without channels."""
 import ctypes as C
 
 import pytest
@@ -106,3 +108,55 @@ def test_layernorm_family_refuses_misaligned_pointers(fn, field, off, extra):
     rc = ln_call(fn, **{field: base[field] + off}, **extra)
     name = {"layernorm16": {"x": "x16", "out": "out16"}}.get(fn, {}).get(field, field)
     expect_refused(rc, name)
+
+
+def ptrs(*addrs):
+    return (C.c_void_p * len(addrs))(*addrs)
+
+
+def elementwise_call(fn, field, off):
+    """One vectorised elementwise entry point with aligned made-up pointers, `field` moved by `off` bytes."""
+    L = lib()
+    at = lambda f, a: a + off if f == field else a                          # noqa: E731
+    if fn == "im2col16":
+        return L.m3r_im2col16(at("img", BASE), 2, 32, 48, at("out", BASE + 0x100000), 0, None)
+    if fn == "attn_merge":
+        po = ptrs(BASE, BASE + 0x10000, at("parts_o[2]", BASE + 0x20000))
+        pml = ptrs(BASE + 0x30000, at("parts_ml[1]", BASE + 0x40000), BASE + 0x50000)
+        return L.m3r_attn_merge(po, pml, 3, 64, 2, at("out", BASE + 0x60000), 128, 0, None)
+    if fn == "attn_state_fill":
+        return L.m3r_attn_state_fill(at("export_o", BASE), at("export_ml", BASE + 0x10000), 64, 2, None)
+    d = ptrs(BASE + 0x10000, BASE + 0x20000, at("dsts[2]", BASE + 0x30000))
+    return L.m3r_peer_bcast(at("src", BASE), d, 3, 4096, None)
+
+
+@pytest.mark.parametrize("fn,field,off", [
+    ("im2col16", "img", 8), ("im2col16", "img", 4), ("im2col16", "out", 4), ("im2col16", "out", 2),
+    ("attn_merge", "parts_o[2]", 8), ("attn_merge", "parts_ml[1]", 4), ("attn_merge", "out", 8),
+    ("attn_state_fill", "export_o", 8), ("attn_state_fill", "export_ml", 4),
+    ("peer_bcast", "src", 8), ("peer_bcast", "dsts[2]", 8), ("peer_bcast", "dsts[2]", 4),
+])
+def test_elementwise_refuses_misaligned_pointers(fn, field, off):
+    expect_refused(elementwise_call(fn, field, off), field)
+
+
+def expect_argument_error(rc, *words):
+    msg = last_error()
+    assert rc != 0 and all(w in msg for w in words), (rc, msg)
+
+
+def test_peer_bcast_refuses_a_null_destination():
+    d = ptrs(BASE + 0x10000, None, BASE + 0x30000)
+    expect_argument_error(lib().m3r_peer_bcast(BASE, d, 3, 4096, None), "dsts[1]", "non-null")
+
+
+@pytest.mark.parametrize("B,N,H,D", [(-1, -2, 3, 64), (2, -3, -1, 64), (-2, 5, -4, 12), (1, 1, 1, -4)])
+def test_rope_2d_refuses_negative_dimensions(B, N, H, D):
+    rc = lib().m3r_rope_2d(BASE, 1, B, N, H, D, 4096, 64, 64, BASE + 0x100000, 100.0, 1.0, None)
+    expect_argument_error(rc, "rope_2d", "negative dimension")
+
+
+@pytest.mark.parametrize("C_", [0, -1, -7])
+def test_unpatchify_refuses_no_channels(C_):
+    rc = lib().m3r_unpatchify(BASE, 2, 32, 48, C_, BASE + 0x100000, None)
+    expect_argument_error(rc, "unpatchify", "C=")
