@@ -197,6 +197,14 @@ typedef struct {
 } m3r_attn_args;
 
 int m3r_attention(const m3r_attn_args* args, void* stream);
+/* Ragged form: K/V batch k (of B / kv_group) attends to rows j < nk0_b[k] of segment 0 only; nk0_b is an int32 device
+ * array [B / kv_group] read by the kernel, its values clamped to [0, Nk0], and Nk0 (>= 1) is the longest batch: the length
+ * the tensor maps and the key splits are planned for.  Rows at or past a batch's own length may hold anything (NaN and inf
+ * included) and influence no output bit.  Segment 1 and the skip range keep their meaning (segment 1's global index is
+ * Nk0 + j for every batch).  Equal lengths give bitwise the result of m3r_attention.  Export mode is an argument error.
+ * The lengths are only known on the device, so a batch left with no key at all cannot be refused: its rows come out 0.
+ * Used by the decoder call over several SLAM sessions (m3r_decoder_forward_ragged), whose memories differ in length. */
+int m3r_attention_ragged(const m3r_attn_args* args, const int32_t* nk0_b, void* stream);
 
 /* Merge `n` exported attention states of the same queries over disjoint key sets:
  * out[r, c] = sum_k o_k[r, c] 2^(m_k[r,h] - m) / sum_k l_k[r,h] 2^(m_k[r,h] - m), m = max_k m_k, h = c / 64.
@@ -471,6 +479,26 @@ int m3r_peer_wait(const void* local_flags, uint32_t rank_mask, uint32_t value, v
 /* MUSt3R.forward / forward_list (decoder.py:158-350) for memory_mode 'kv'. */
 int m3r_decoder_forward(const m3r_decoder_weights* w, const m3r_decoder_call* call, void* workspace,
                         int64_t workspace_bytes, void* stream);
+
+/* The same memory update over B scenes whose memories hold different numbers of tokens (several SLAM sessions stepped
+ * together, must3r_b200/engine/slam_sessions.py): scene b attends to rows [0, nm_scene[b]) of its memory, nm_scene an
+ * int32 device array [B] (values clamped to [0, call->Nm]); call->Nm is the longest memory and must be >= 1, and each
+ * scene's memory rows begin at b * mem_bstride_rows.  Every layer's memory cross-attention runs as m3r_attention_ragged.
+ * Only memory_mode kv with new_only = 1 (no render, no peers, no context parallel): the new post-feedback K|V rows of
+ * every scene go to mem_out[l] [B, Nt, 2D] and nothing is written into the memory; m3r_mem_commit appends them.  The
+ * workspace is m3r_decoder_workspace_bytes(w, call). */
+int m3r_decoder_forward_ragged(const m3r_decoder_weights* w, const m3r_decoder_call* call, const int32_t* nm_scene,
+                               void* workspace, int64_t workspace_bytes, void* stream);
+
+/* Keyframe commit of several SLAM sessions in one launch: for each scene b < B whose flag keep[b * keep_stride] (int32,
+ * device; e.g. the keyframe field of its m3r_slam_record) is non-zero, copy rows [0, Nt) of staged[l] + b * Nt * width
+ * (the [B, Nt, width] 16-bit new_only output of m3r_decoder_forward_ragged) to rows dst_row[b] .. dst_row[b] + Nt - 1 of
+ * arena[l] (rows of `width` 16-bit elements), for every level l < depth.  A scene whose flag is zero writes nothing.
+ * arena, staged: host arrays [depth] of device pointers; dst_row: host array [B].  B <= M3R_MAX_COMMIT,
+ * depth <= M3R_MAX_GROUPS, width % 8 == 0, every arena / staged pointer 16-byte aligned and keep 4-byte aligned. */
+#define M3R_MAX_COMMIT 64
+int m3r_mem_commit(void* const* arena, const void* const* staged, int32_t depth, int32_t B, int32_t Nt, int32_t width,
+                   const int64_t* dst_row, const int32_t* keep, int64_t keep_stride, void* stream);
 
 
 #ifdef __cplusplus

@@ -77,6 +77,9 @@ SIGNATURES = {
     "m3r_rope_2d": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_int64,
                               C.c_int64, C.c_void_p, C.c_float, C.c_float, C.c_void_p]),
     "m3r_attention": (C.c_int, [C.POINTER(AttnArgs), C.c_void_p]),
+    "m3r_attention_ragged": (C.c_int, [C.POINTER(AttnArgs), C.c_void_p, C.c_void_p]),
+    "m3r_mem_commit": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                 C.POINTER(C.c_int64), C.c_void_p, C.c_int64, C.c_void_p]),
     "m3r_attn_merge": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int32, C.c_int64, C.c_int32, C.c_void_p, C.c_int64,
                                  C.c_int32, C.c_void_p]),
     "m3r_attn_state_fill": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p]),

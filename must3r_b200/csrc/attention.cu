@@ -26,6 +26,13 @@
 // masked key tiles are never loaded.  Small grids (one view per step) split the key range over several CTAs; the
 // last CTA to finish a (batch, head, 64-row query tile) merges the partial (O, m, l) in-kernel.  The split
 // count comes from a wave-count cost model (m3r_attention).
+//
+// Ragged segment 0 (m3r_attention_ragged): K/V batch b attends to rows j < nk0_b[b] of segment 0 only (the memories of
+// several SLAM sessions, each of its own length, behind one decoder call).  The tensor maps span the longest batch, so the
+// tiles of a shorter batch are enumerated from its own length and its last partial tile loads real rows behind its end.
+// Their scores are masked like any padding; their V rows are zeroed in shared memory before P V, because P = 0 times a
+// stale NaN / inf V element is still NaN.  Splits are planned for the longest batch; each batch divides its own tiles
+// over them, and a CTA left without a tile contributes the empty state (m = -inf, l = 0) to the merge.
 #include <math.h>
 #include "ptx.cuh"
 #include "m3r_internal.h"
@@ -61,6 +68,7 @@ struct AttnParams {
   int kv_group;
   int skip_lo, skip_step, skip_len;
   int splits;                // key-range splits (>=1); blockIdx.z = b * splits + split
+  const int* nk0_b;          // ragged: [B / kv_group] segment-0 lengths, clamped to [0, Nk0]; null = Nk0 for every batch
   float sl2;                 // scale * log2(e)
   void* O;                   // [B*Nq, H*64] 16-bit                     (splits == 1)
   long long ldo;
@@ -89,7 +97,7 @@ struct TileIt {
 // tile index (segment 0 tiles, then segment 1 tiles), so tile i of the visit is linear tile i (+ ns past the run).
 // Every warp role maps indices the same way; no per-thread walk over the (possibly thousands of) tiles.
 struct TileMap {
-  int nk0, nk1, lo, hi;
+  int nk0, base1, nk1, lo, hi;      // base1: global index of segment 1's first key (Nk0 of the call, >= nk0 when ragged)
   int T0, s0, ns, n_all;
   __device__ static void masked_run(int n, int base, int T, int lo, int hi, int& a, int& c) {
     const int l = lo - base, h = hi - base;
@@ -97,13 +105,13 @@ struct TileMap {
     const int b = h >= n ? T : (h <= 0 ? 0 : h / AT_BN);       // one past the last tile with g1 <= hi
     c = max(0, min(b, T) - a);
   }
-  __device__ TileMap(int nk0_, int nk1_, int lo_, int hi_) : nk0(nk0_), nk1(nk1_), lo(lo_), hi(hi_) {
+  __device__ TileMap(int nk0_, int base1_, int nk1_, int lo_, int hi_) : nk0(nk0_), base1(base1_), nk1(nk1_), lo(lo_), hi(hi_) {
     T0 = (nk0 + AT_BN - 1) / AT_BN;
     const int T1 = (nk1 + AT_BN - 1) / AT_BN;
     int a0 = 0, c0 = 0, a1 = 0, c1 = 0;
     if (hi > lo) {
       masked_run(nk0, 0, T0, lo, hi, a0, c0);
-      masked_run(nk1, nk0, T1, lo, hi, a1, c1);
+      masked_run(nk1, base1, T1, lo, hi, a1, c1);
     }
     s0 = c0 > 0 ? a0 : T0 + a1;       // (a range covering both segments ends segment 0 and starts segment 1: contiguous)
     ns = c0 + c1;
@@ -117,7 +125,7 @@ struct TileMap {
     const int n = it.seg ? nk1 : nk0;
     const int l0 = it.t * AT_BN;
     it.nvalid = min(AT_BN, n - l0);
-    it.g0 = (it.seg ? nk0 : 0) + l0;
+    it.g0 = (it.seg ? base1 : 0) + l0;
     it.mask = (it.nvalid < AT_BN) || (it.g0 < hi && it.g0 + it.nvalid > lo);
     return it;
   }
@@ -200,6 +208,18 @@ template <bool BF16> __device__ __forceinline__ void issue_pv(float (&o)[32], co
   }
 }
 
+// Ragged batch, last partial tile of segment 0: zero the V rows [nvalid, 128) of the stage (rows of another, longer batch's
+// length that TMA did load) so that P V reads exact zeros there.  SW128 keeps each 128-byte row in place, so the rows
+// are one contiguous byte range.  Every consumer thread of both warpgroups takes part, then the generic-proxy stores
+// are made visible to wgmma and the warpgroups meet before either multiplies the stage.
+template <int CT> __device__ __forceinline__ void zero_v_tail(uint8_t* sv, int nvalid) {
+  uint4* v = reinterpret_cast<uint4*>(sv + nvalid * HD * 2);
+  const int n = (AT_BN - nvalid) * (HD * 2 / 16);
+  for (int i = threadIdx.x; i < n; i += CT) v[i] = make_uint4(0u, 0u, 0u, 0u);
+  fence_proxy_async_smem();
+  asm volatile("bar.sync 1, %0;" ::"n"(CT) : "memory");
+}
+
 template <bool BF16>
 __global__ void __launch_bounds__(AttnCfg::THREADS, 1)
 attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK0,
@@ -232,14 +252,6 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
   const int hi = p.skip_len > 0 ? lo + p.skip_len : 0;
   const int q0 = blockIdx.x * NWG * AT_BM;
 
-  // this CTA's share [i0, i1) of the enumerated key tiles
-  const TileMap tiles(p.Nk0, p.Nk1, lo, hi);
-  const int n_all = tiles.n_all;
-  const int chunk = (n_all + p.splits - 1) / p.splits;
-  const int i0 = split * chunk;
-  const int i1 = min(n_all, i0 + chunk);
-  const int n_tiles = max(i1 - i0, 0);
-
   if (warp == TMA_WARP && elect_one()) {
     tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK0); tma_prefetch_desc(&tmV0);
     if (p.Nk1 > 0) { tma_prefetch_desc(&tmK1); tma_prefetch_desc(&tmV1); }
@@ -250,6 +262,16 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
   __syncthreads();
   griddep_wait();
   griddep_launch();
+
+  // this CTA's share [i0, i1) of the enumerated key tiles (the ragged lengths may come from the preceding kernel: read
+  // after the dependency wait)
+  const int nk0 = p.nk0_b ? min(max(__ldg(p.nk0_b + kvb), 0), p.Nk0) : p.Nk0;
+  const TileMap tiles(nk0, p.Nk0, p.Nk1, lo, hi);
+  const int n_all = tiles.n_all;
+  const int chunk = (n_all + p.splits - 1) / p.splits;
+  const int i0 = split * chunk;
+  const int i1 = min(n_all, i0 + chunk);
+  const int n_tiles = max(i1 - i0, 0);
 
   if (wg == NWG) {
     // ------------------------------------------------------------------ TMA producer warpgroup
@@ -310,6 +332,10 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
       M3R_TR(if (tr && j < 12) tr[8 + 4 * j] = gtime_ns();)
       mbar_wait(&k_full[st], (j / KS) & 1);
       mbar_wait(&v_full[pst], ((j - 1) / KS) & 1);
+      if (p.nk0_b) {
+        const TileIt pt = tiles.get(i0 + j - 1);
+        if (pt.seg == 0 && pt.nvalid < AT_BN) zero_v_tail<CT>(sV + pst * TILE_BYTES, pt.nvalid);
+      }
       wgmma_fence();
       issue_qk<BF16>(s, qdesc, smem_desc_sw128(smem_u32(sK + st * TILE_BYTES)));
       wgmma_commit();
@@ -329,6 +355,10 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
     }
     const int lst = (n_tiles - 1) % KS;
     mbar_wait(&v_full[lst], ((n_tiles - 1) / KS) & 1);
+    if (p.nk0_b) {
+      const TileIt pt = tiles.get(i0 + n_tiles - 1);
+      if (pt.seg == 0 && pt.nvalid < AT_BN) zero_v_tail<CT>(sV + lst * TILE_BYTES, pt.nvalid);
+    }
     wgmma_fence();
     issue_pv<BF16>(o, pa, smem_desc_sw128(smem_u32(sV + lst * TILE_BYTES)));
     wgmma_commit();
@@ -507,11 +537,8 @@ static int launch_attn(const CUtensorMap& tmQ, const CUtensorMap& tmK0, const CU
   return 0;
 }
 
-}  // namespace m3r
 
-// Number of fp32 scratch elements m3r_attention may need for a problem (0 if it will not split).
-extern "C" int m3r_attention(const m3r_attn_args* a, void* stream) {
-  using namespace m3r;
+static int attention(const m3r_attn_args* a, const int32_t* nk0_b, void* stream) {
   if (!a || !a->Q || !a->K0 || !a->V0 || (!a->O && !a->export_o)) return set_error("attention: null pointer");
   if ((a->export_o == nullptr) != (a->export_ml == nullptr)) return set_error("attention: export_o and export_ml go together");
   if (a->B <= 0 || a->H <= 0 || a->Nq <= 0) return 0;
@@ -569,7 +596,7 @@ extern "C" int m3r_attention(const m3r_attn_args* a, void* stream) {
   AttnParams p;
   p.Nq = a->Nq; p.Nk0 = a->Nk0; p.Nk1 = a->Nk1; p.kv_group = a->kv_group;
   p.skip_lo = a->skip_lo; p.skip_step = a->skip_step; p.skip_len = a->skip_len;
-  p.splits = splits; p.sl2 = a->scale * 1.4426950408889634f;
+  p.splits = splits; p.sl2 = a->scale * 1.4426950408889634f; p.nk0_b = nk0_b;
   p.O = a->O; p.ldo = a->ldo; p.H = a->H; p.rows_total = (long long)a->B * a->Nq;
   p.part_o = nullptr; p.part_ml = nullptr; p.split_cnt = nullptr;
   p.exp_o = a->export_o; p.exp_ml = reinterpret_cast<float2*>(a->export_ml);
@@ -606,4 +633,16 @@ extern "C" int m3r_attention(const m3r_attn_args* a, void* stream) {
     if (rc) return rc;
   }
   return 0;
+}
+}  // namespace m3r
+
+extern "C" int m3r_attention(const m3r_attn_args* a, void* stream) { return m3r::attention(a, nullptr, stream); }
+
+extern "C" int m3r_attention_ragged(const m3r_attn_args* a, const int32_t* nk0_b, void* stream) {
+  using namespace m3r;
+  if (!nk0_b) return set_error("attention_ragged: null nk0_b");
+  if (reinterpret_cast<uintptr_t>(nk0_b) % 4) return set_error("attention_ragged: nk0_b must be 4-byte aligned");
+  if (a && (a->export_o || a->export_ml)) return set_error("attention_ragged: export mode is not supported with ragged lengths");
+  if (a && a->Nk0 < 1) return set_error("attention_ragged: Nk0 (the longest batch, %d) must be >= 1", a->Nk0);
+  return attention(a, nk0_b, stream);
 }

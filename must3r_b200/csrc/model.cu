@@ -10,8 +10,10 @@
 //   decoder only     snap   fp32  [depth][M,D]  block inputs (= new_mem[l], decoder.py:304) kept for the feedback
 //                    kvnew  16b   [B, Nt, 2D]   this step's pre-feedback K|V (second key segment of the CA)
 #include <stdio.h>
+#include <algorithm>
 #include <vector>
 #include "m3r_internal.h"
+#include "ptx.cuh"
 
 namespace m3r {
 
@@ -213,8 +215,11 @@ extern "C" int64_t m3r_decoder_workspace_bytes(const m3r_decoder_weights* w, con
   return dec_layout(w, c, nullptr, 0, &ws);
 }
 
-extern "C" int m3r_decoder_forward(const m3r_decoder_weights* w, const m3r_decoder_call* c, void* workspace,
-                                   int64_t workspace_bytes, void* stream) {
+namespace m3r {
+
+// nm_scene != null: the ragged update of m3r_decoder_forward_ragged (checked there)
+static int decoder_forward(const m3r_decoder_weights* w, const m3r_decoder_call* c, const int32_t* nm_scene,
+                           void* workspace, int64_t workspace_bytes, void* stream) {
   if (!w || !c || !workspace || !c->groups) return set_error("decoder_forward: null pointer");
   if (c->B <= 0 || c->G <= 0) return set_error("decoder_forward: empty call");
   if (w->embed_dim != w->num_heads * 64) return set_error("decoder_forward: head_dim must be 64");
@@ -470,7 +475,7 @@ extern "C" int m3r_decoder_forward(const m3r_decoder_weights* w, const m3r_decod
       at.O = ws.att16 + ws.row0[g] * D; at.ldo = D; at.B = B * gr.n_views; at.H = Hh; at.Nq = gr.N;
       at.kv_group = gr.n_views; at.is_bf16 = bf; at.scale = 0.125f;
       if (use_skip && at.Nk0 + at.Nk1 > (Nm > 0 ? Nm : 0) ) { at.skip_lo = Nm + (int)ws.tok0[g]; at.skip_step = gr.N; at.skip_len = gr.N; }
-      M3R_TRY(m3r_attention(&at, stream));
+      M3R_TRY(nm_scene ? m3r_attention_ragged(&at, nm_scene, stream) : m3r_attention(&at, stream));
     }
     if (cp) {
       // exchange: my state -> slot cp_rank of every rank's staging buffer (parity alternates so that a rank one layer ahead
@@ -511,5 +516,68 @@ extern "C" int m3r_decoder_forward(const m3r_decoder_weights* w, const m3r_decod
     if (Nm > 0 && !c->new_only) M3R_TRY(link(sd, sd->copy, cs));    // and the old-memory copies
   }
   join_guard.done = true;
+  return 0;
+}
+
+struct CommitArgs {
+  uint4* dst[M3R_MAX_GROUPS];
+  const uint4* src[M3R_MAX_GROUPS];
+  long long dst_row[M3R_MAX_COMMIT];
+};
+
+// grid (chunks, B, depth): level blockIdx.z of scene blockIdx.y, if its flag is set; rows * width / 8 uint4 per scene
+__global__ void mem_commit_kernel(const __grid_constant__ CommitArgs a, const int* keep, long long keep_stride, int Nt, int w16) {
+  griddep_wait();
+  const int b = blockIdx.y, l = blockIdx.z;
+  if (keep[(long long)b * keep_stride] == 0) return;
+  const long long n = (long long)Nt * w16;
+  const uint4* src = a.src[l] + (long long)b * n;
+  uint4* dst = a.dst[l] + a.dst_row[b] * w16;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) dst[i] = src[i];
+}
+
+}  // namespace m3r
+
+extern "C" int m3r_decoder_forward(const m3r_decoder_weights* w, const m3r_decoder_call* c, void* workspace,
+                                   int64_t workspace_bytes, void* stream) {
+  return decoder_forward(w, c, nullptr, workspace, workspace_bytes, stream);
+}
+
+extern "C" int m3r_decoder_forward_ragged(const m3r_decoder_weights* w, const m3r_decoder_call* c, const int32_t* nm_scene,
+                                          void* workspace, int64_t workspace_bytes, void* stream) {
+  if (!c || !nm_scene) return set_error("decoder_forward_ragged: null pointer");
+  if (c->mem_mode != M3R_MEM_KV || !c->new_only || c->render || c->n_peers != 0 || c->cp_world > 1)
+    return set_error("decoder_forward_ragged: only memory_mode kv with new_only (no render, peers or context parallel)");
+  if (c->Nm < 1 || c->is_init) return set_error("decoder_forward_ragged: needs a memory (Nm = the longest, >= 1)");
+  return decoder_forward(w, c, nm_scene, workspace, workspace_bytes, stream);
+}
+
+extern "C" int m3r_mem_commit(void* const* arena, const void* const* staged, int32_t depth, int32_t B, int32_t Nt, int32_t width,
+                              const int64_t* dst_row, const int32_t* keep, int64_t keep_stride, void* stream) {
+  if (!arena || !staged || !dst_row || !keep) return set_error("mem_commit: null pointer");
+  if (B < 0 || B > M3R_MAX_COMMIT || depth < 1 || depth > M3R_MAX_GROUPS || Nt < 0 || width < 8 || width % 8)
+    return set_error("mem_commit: B in [0, %d], depth in [1, %d], Nt >= 0 and width a positive multiple of 8", M3R_MAX_COMMIT, M3R_MAX_GROUPS);
+  if (reinterpret_cast<uintptr_t>(keep) % 4) return set_error("mem_commit: keep must be 4-byte aligned");
+  CommitArgs a = {};
+  for (int l = 0; l < depth; ++l) {
+    if (!arena[l] || !staged[l] || reinterpret_cast<uintptr_t>(arena[l]) % 16 || reinterpret_cast<uintptr_t>(staged[l]) % 16)
+      return set_error("mem_commit: arena[%d] / staged[%d] null or not 16-byte aligned", l, l);
+    a.dst[l] = reinterpret_cast<uint4*>(arena[l]);
+    a.src[l] = reinterpret_cast<const uint4*>(staged[l]);
+  }
+  for (int b = 0; b < B; ++b) {
+    if (dst_row[b] < 0) return set_error("mem_commit: dst_row[%d] < 0", b);
+    a.dst_row[b] = dst_row[b];
+  }
+  if (B == 0 || Nt == 0) return 0;
+  const int w16 = width / 8;
+  const long long n = (long long)Nt * w16;
+  const int threads = 256;
+  const int chunks = (int)std::min<long long>((n + threads - 1) / threads, 64);
+  cudaError_t e = launch_pdl(mem_commit_kernel, dim3(chunks, B, depth), dim3(threads), 0, reinterpret_cast<cudaStream_t>(stream),
+                             a, keep, (long long)keep_stride, (int)Nt, w16);
+  if (e == cudaSuccess) e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error("mem_commit launch: %s", cudaGetErrorString(e));
+  count_launch();
   return 0;
 }

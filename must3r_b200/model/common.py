@@ -69,6 +69,8 @@ _lib.SIGNATURES.update({
     "m3r_decoder_workspace_bytes": (C.c_int64, [C.POINTER(DecoderWeights), C.POINTER(DecoderCall)]),
     "m3r_decoder_cp_slot_bytes": (C.c_int64, [C.POINTER(DecoderWeights), C.c_int64]),
     "m3r_decoder_forward": (C.c_int, [C.POINTER(DecoderWeights), C.POINTER(DecoderCall), C.c_void_p, C.c_int64, C.c_void_p]),
+    "m3r_decoder_forward_ragged": (C.c_int, [C.POINTER(DecoderWeights), C.POINTER(DecoderCall), C.c_void_p, C.c_void_p,
+                                             C.c_int64, C.c_void_p]),
 })
 
 _lib.apply_signatures()

@@ -232,11 +232,17 @@ class MUSt3R(nn.Module):
         return mem, pms[0]
 
     @torch.no_grad()
-    def update_tokens(self, x, pos, true_shape, current_mem=None):
+    def update_tokens(self, x, pos, true_shape, current_mem=None, mem_lengths=None):
         """Memory-update call that returns only this call's new post-feedback K|V tokens
         (list[depth] of [B, n*N, 2D]) and the raw pointmaps, instead of the concatenated memory
-        (= ``mem'[0][l][:, Nm:]`` of ``forward``).  Used by the sharded multi-GPU schedule (SURVEY.md §8e)."""
-        _, pms, new_tokens = self.forward_list([x], [pos], [true_shape], current_mem, render=False, _new_only=True)
+        (= ``mem'[0][l][:, Nm:]`` of ``forward``).  Used by the sharded multi-GPU schedule (SURVEY.md §8e).
+
+        ``mem_lengths`` (memory_mode 'kv'): B host integers, scene b's memory being rows [0, mem_lengths[b]) of
+        ``current_mem[0][l][b]`` - e.g. a [B, cap, 2D] arena holding one SLAM session per scene.  The scenes are decoded
+        in one call (csrc/model.cu m3r_decoder_forward_ragged), each attending only to its own rows, exactly as B separate
+        calls would; the lengths travel to the device without a host synchronisation."""
+        _, pms, new_tokens = self.forward_list([x], [pos], [true_shape], current_mem, render=False, _new_only=True,
+                                               _mem_lengths=mem_lengths)
         return new_tokens, pms[0]
 
     @torch.no_grad()
@@ -250,7 +256,7 @@ class MUSt3R(nn.Module):
 
     @torch.no_grad()
     def forward_list(self, x, pos, true_shape, current_mem=None, render=False, return_feats=False, _new_only=False,
-                     _peer_ptrs=None, _cp=None):
+                     _peer_ptrs=None, _cp=None, _mem_lengths=None):
         """decoder.py:158-265.  `_cp` (engine/context_parallel.py): dict(world, rank, owner, stage_ptrs, slot_bytes, flag_slots,
         flags_local, epoch0) - the memory is sharded over `world` GPUs and `current_mem` is this rank's shard."""
         if not x[0].is_cuda:
@@ -303,6 +309,17 @@ class MUSt3R(nn.Module):
         else:
             mem_vals, labels, mem_nimgs, mem_pi, mem_pt = current_mem
             Nm = mem_vals[0].shape[1]
+        nm_scene = None
+        if _mem_lengths is not None:
+            lengths = [int(n) for n in _mem_lengths]
+            if self.memory_mode != "kv" or not _new_only or current_mem is None or _peer_ptrs or _cp is not None:
+                raise ValueError("mem_lengths needs memory_mode='kv', a memory and update_tokens")
+            if len(lengths) != B or min(lengths) < 0 or max(lengths) < 1 or max(lengths) > Nm:
+                raise ValueError(f"mem_lengths {lengths}: one length in [0, {Nm}] per scene ({B}), the longest >= 1")
+            Nm = max(lengths)
+            mem_vals = [m[:, :Nm] for m in mem_vals]
+            nm_scene = torch.tensor(lengths, dtype=torch.int32).pin_memory().to(dev, non_blocking=True)
+            keep.append(nm_scene)
         call.Nm = Nm
         mem_ptrs = (C.c_void_p * self.depth)()
         if Nm > 0:
@@ -358,8 +375,13 @@ class MUSt3R(nn.Module):
         nbytes = lib.m3r_decoder_workspace_bytes(C.byref(w), C.byref(call))
         with torch.cuda.device(dev):           # the library keys its per-stream state (side streams, scratch) on the current device
             ws = cm.workspace(dev, nbytes, "dec")
-            _lib.check(lib.m3r_decoder_forward(C.byref(w), C.byref(call), C.c_void_p(ws.data_ptr()), ws.numel(), cm.stream_ptr(dev)),
-                       "decoder_forward")
+            if nm_scene is None:
+                _lib.check(lib.m3r_decoder_forward(C.byref(w), C.byref(call), C.c_void_p(ws.data_ptr()), ws.numel(),
+                                                   cm.stream_ptr(dev)), "decoder_forward")
+            else:
+                _lib.check(lib.m3r_decoder_forward_ragged(C.byref(w), C.byref(call), C.c_void_p(nm_scene.data_ptr()),
+                                                          C.c_void_p(ws.data_ptr()), ws.numel(), cm.stream_ptr(dev)),
+                           "decoder_forward_ragged")
         if _new_only:
             return None, outs, new_mem
         if render:
