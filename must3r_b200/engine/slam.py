@@ -5,7 +5,10 @@ After the decoder call a frame costs two kernels of csrc/slam.cu and one wait: `
 in-place depth rectification, weighted Procrustes, confidence mean and median), the quadrant ids and grid query of the
 keyframe searcher (engine/keyframes.py), `m3r_slam_keyframe` (overlap percentile and keyframe decision), then one
 asynchronous device-to-host copy of the frame's record and of the arrays `__call__` returns, and one wait for it.  A frame
-that is not a keyframe synchronises nowhere else; a keyframe also adds its confident points to the searcher.
+that is not a keyframe synchronises nowhere else; a keyframe also adds its confident points to the searcher.  The tail
+comes in two halves around that wait, `_launch_tail` and `_finish_tail` (on the agent: `launch_tail` / `finish_tail`), and
+`SLAM_MUSt3R._record_frame` does the frame's host bookkeeping, so that engine/slam_sessions.py can put one wait behind
+several sessions' tails.
 
 The decoder computes a memory update for every frame; a frame that is not a keyframe gives the rows it appended back
 (`_release_tail`), so the next update appends in place onto the memory that was kept.
@@ -80,10 +83,11 @@ def mean_focal(seq_focals):
     return (f * c / c.sum()).sum()
 
 
-def _pose_record(res, seq_focal, is_first_frame=False, rectify=True):
-    """m3r_slam_pose over the views of res (pts3d, pts3d_local, conf [1,B,H,W,...]): device records [B, 160]."""
+def _pose_record(res, seq_focal, is_first_frame=False, rectify=True, rec=None):
+    """m3r_slam_pose over the views of res (pts3d, pts3d_local, conf [1,B,H,W,...]): device records [B, 160] (into
+    `rec` if given)."""
     return ops.slam_pose(res['pts3d'][0], res['pts3d_local'][0], res['conf'][0],
-                         seq_focal=seq_focal if rectify else None, is_first=is_first_frame)
+                         seq_focal=seq_focal if rectify else None, is_first=is_first_frame, rec=rec)
 
 
 def get_camera_pose(res, seq_focal, HW, is_first_frame=False, rectify=True):
@@ -120,41 +124,55 @@ def _index_ready(tree, device):
             grid._build(torch.device(device))
 
 
+def _launch_tail(img, res, is_first_frame, seq_focal, overlap_mode, overlap_tree, kf_x_subsamp, keyframe_overlap_thr,
+                 min_conf_keyframe, overlap_percentile, img_mean, img_std, rec=None):
+    """The device half of postproc_pred, which never waits: m3r_slam_pose into `rec` (a new [1, 160] record unless
+    given, e.g. a row of a batch of records), the searcher query, m3r_slam_keyframe and the asynchronous host copies of
+    the point map and the colours.  -> the tail that _finish_tail takes once the record is on the host."""
+    assert res['pts3d'].shape[0] == 1 and res['pts3d'].shape[1] == 1, "frames come one by one here"
+    conf = res['conf'][0, 0]
+    s = kf_x_subsamp or 1
+    rec = _pose_record(res, seq_focal, is_first_frame, rec=rec)
+    c2w = ops.slam_record_c2w(rec)[0]
+    sub = res['pts3d'][0, 0, ::s, ::s].reshape(-1, 3)
+    dists = None
+    if ops.overlap_mode_id(overlap_mode) <= 1:
+        dists = overlap_tree.query(sub, cam_center=c2w[:3, -1]).float().contiguous()
+    ops.slam_keyframe(dists, conf, res['pts3d_local'][0, 0], rec, subsamp=s, mode=overlap_mode,
+                      percentile=overlap_percentile, thr=keyframe_overlap_thr, min_conf_keyframe=min_conf_keyframe,
+                      is_first=bool(is_first_frame))
+    cols = prep_imgs(img['img'], img_mean=img_mean, img_std=img_std)[None]
+    host = [_to_out(t, 'cpu') for t in (res['pts3d'][0, 0], cols)]
+    return rec, c2w, sub, conf[::s, ::s], min_conf_keyframe, host
+
+
+def _finish_tail(res, tail, r):
+    """The host half of postproc_pred: the launched `tail` and the frame's host record r -> postproc_pred's tuple; sets
+    res['overlap_score'], res['slam_record'] (r) and res['slam_c2w'] (the pose on the device)."""
+    rec, c2w, sub, conf_sub, min_conf_keyframe, host = tail
+    # the confident subsampled points, in pixel order: a stable sort of the mask puts them first (no host sync)
+    msk = conf_sub.reshape(-1) > min_conf_keyframe
+    pts = sub[torch.argsort((~msk).to(torch.uint8), stable=True)[:int(r['n_conf'])]]
+    res['overlap_score'] = float(r['score'])
+    res['slam_record'] = r
+    res['slam_c2w'] = c2w
+    w2c = rec[0, 64:128].view(torch.float32).view(4, 4)
+    return (pts, host[0], host[1], res['pts3d_local'][0, 0, ..., -1], res['conf'][0, 0],
+            np.array([r['focal']], dtype=np.float32), w2c, c2w[:3, -1], bool(r['keyframe']))
+
+
 def postproc_pred(img, res, is_first_frame, seq_focals, fixed_focal=True, overlap_mode='nn-norm', overlap_tree=None,
                   kf_x_subsamp=None, keyframe_overlap_thr=.15, min_conf_keyframe=1.5, overlap_percentile=70,
                   img_mean=[0.5, 0.5, 0.5], img_std=[0.5, 0.5, 0.5]):
     """must3r/slam/model.py:185-248 -> (pts, allpts, cols, depth, conf, focal, w2c, cam_center, iskeyframe).
     Reads the frame's record back once; also sets res['overlap_score'], res['slam_record'] (the host record) and
     res['slam_c2w'] (the pose on the device)."""
-    assert res['pts3d'].shape[0] == 1 and res['pts3d'].shape[1] == 1, "frames come one by one here"
-    depth = res['pts3d_local'][0, 0, ..., -1]
-    conf = res['conf'][0, 0]
-    s = kf_x_subsamp or 1
     seq_focal = mean_focal(seq_focals) if fixed_focal else None
-    rec = _pose_record(res, seq_focal, is_first_frame)
-    c2w = ops.slam_record_c2w(rec)[0]
-    cam_center = c2w[:3, -1]
-    sub = res['pts3d'][0, 0, ::s, ::s].reshape(-1, 3)
-    dists = None
-    if ops.overlap_mode_id(overlap_mode) <= 1:
-        dists = overlap_tree.query(sub, cam_center=cam_center).float().contiguous()
-    ops.slam_keyframe(dists, conf, res['pts3d_local'][0, 0], rec, subsamp=s, mode=overlap_mode,
-                      percentile=overlap_percentile, thr=keyframe_overlap_thr, min_conf_keyframe=min_conf_keyframe,
-                      is_first=bool(is_first_frame))
-    allpts = res['pts3d'][0, 0]
-    cols = prep_imgs(img['img'], img_mean=img_mean, img_std=img_std)[None]
-    host = [_to_out(t, 'cpu') for t in (rec, allpts, cols)]
+    tail = _launch_tail(img, res, is_first_frame, seq_focal, overlap_mode, overlap_tree, kf_x_subsamp,
+                        keyframe_overlap_thr, min_conf_keyframe, overlap_percentile, img_mean, img_std)
+    host_rec = _to_out(tail[0], 'cpu')
     _wait_host_copies()
-    r = host[0].numpy().view(ops.SLAM_RECORD)[0, 0]
-    # the confident subsampled points, in pixel order: a stable sort of the mask puts them first (no host sync)
-    msk = conf[::s, ::s].reshape(-1) > min_conf_keyframe
-    pts = sub[torch.argsort((~msk).to(torch.uint8), stable=True)[:int(r['n_conf'])]]
-    res['overlap_score'] = float(r['score'])
-    res['slam_record'] = r
-    res['slam_c2w'] = c2w
-    w2c = rec[0, 64:128].view(torch.float32).view(4, 4)
-    return (pts, host[1], host[2], depth, conf, np.array([r['focal']], dtype=np.float32), w2c, cam_center,
-            bool(r['keyframe']))
+    return _finish_tail(res, tail, host_rec.numpy().view(ops.SLAM_RECORD)[0, 0])
 
 
 class MUSt3R_Agent():
@@ -181,20 +199,35 @@ class MUSt3R_Agent():
             return mean_focal(self.seq_focals) * to_orig[0]
         return [f * t for f, t in zip(self.seq_focals['f'], self.seq_focals['to_orig'])]
 
+    def add_focal(self, r, to_orig_focal):
+        """Record the focal and confidence of a frame's host record r -> the focal the frame reports: the weighted mean
+        so far (fixed focal) or its own."""
+        self.seq_focals['f'].append(np.float32(r['focal']))
+        self.seq_focals['to_orig'].append(to_orig_focal)
+        self.seq_focals['conf'].append(np.float32(r['conf_mean']) - 1.)
+        return mean_focal(self.seq_focals) if self.fixed_focal else self.seq_focals['f'][-1]
+
+    def launch_tail(self, inp, pred, is_first_frame, overlap_mode, overlap_tree, kf_x_subsamp, keyframe_overlap_thr,
+                    min_conf_keyframe, overlap_percentile, rec=None):
+        """The device half of `update` (it never waits), with this agent's focal; `rec` as in _launch_tail."""
+        return _launch_tail(inp, pred, is_first_frame, mean_focal(self.seq_focals) if self.fixed_focal else None,
+                            overlap_mode, overlap_tree, kf_x_subsamp, keyframe_overlap_thr, min_conf_keyframe,
+                            overlap_percentile, self.img_mean, self.img_std, rec=rec)
+
+    def finish_tail(self, pred, tail, r, to_orig_focal):
+        """The host half of `update` once the frame's record r is on the host -> update's tuple."""
+        out = _finish_tail(pred, tail, r)
+        return out[:5] + (self.add_focal(r, to_orig_focal),) + out[6:]
+
     @torch.no_grad()
     def update(self, inp, pred, is_first_frame, overlap_mode, overlap_tree, kf_x_subsamp, keyframe_overlap_thr,
                min_conf_keyframe, overlap_percentile, to_orig_focal):
-        selpts3d, pts3d, colors, depth, conf, focal, w2c, cam_center, iskeyframe = postproc_pred(
+        out = postproc_pred(
             img=inp, res=pred, is_first_frame=is_first_frame, seq_focals=self.seq_focals, fixed_focal=self.fixed_focal,
             overlap_mode=overlap_mode, overlap_tree=overlap_tree, kf_x_subsamp=kf_x_subsamp,
             keyframe_overlap_thr=keyframe_overlap_thr, min_conf_keyframe=min_conf_keyframe,
             overlap_percentile=overlap_percentile, img_mean=self.img_mean, img_std=self.img_std)
-        r = pred['slam_record']
-        self.seq_focals['f'].append(focal[0])
-        self.seq_focals['to_orig'].append(to_orig_focal)
-        self.seq_focals['conf'].append(np.float32(r['conf_mean']) - 1.)
-        outfocal = mean_focal(self.seq_focals) if self.fixed_focal else self.seq_focals['f'][-1]
-        return selpts3d, pts3d, colors, depth, conf, outfocal, w2c, cam_center, iskeyframe
+        return out[:5] + (self.add_focal(pred['slam_record'], to_orig_focal),) + out[6:]
 
 
 def get_map(ptscolsconfs, confthr):
@@ -215,8 +248,7 @@ class SLAM_MUSt3R():
         self.num_init_frames = num_init_frames
         self.res = res
         self.device = device
-        self.model = load_model(chkpt, device=device)
-        _reserve(self.model[1], 0, 1.5)          # memory buffers grow geometrically: updates append in place
+        self.model = self._load_model(chkpt, device)
         self.searcher = searcher
         self.kf_x_subsamp = kf_x_subsamp
         self.keyframe_overlap_thr = keyframe_overlap_thr
@@ -232,6 +264,11 @@ class SLAM_MUSt3R():
         if load_memory is not None:
             self.load_memory(load_memory)
         self.reset()
+
+    def _load_model(self, chkpt, device):
+        model = load_model(chkpt, device=device)
+        _reserve(model[1], 0, 1.5)               # memory buffers grow geometrically: updates append in place
+        return model
 
     def reset(self):
         """Back to the loaded memory if there is one, else to an empty map."""
@@ -336,24 +373,32 @@ class SLAM_MUSt3R():
         preds, newmem = forward_must3r(self.model, query_images, self.memory, device=self.device)
         kept = False
         for view, pred, fid in zip(query_images, preds, frame_ids):
-            HW = view['true_shape'][0]
-            selpts3d, pts3d, colors, depth, conf, focal, w2c, cam_center, iskeyframe = self.agents[cam_id].update(
+            out = self.agents[cam_id].update(
                 view, pred, self.memory is None, overlap_mode=self.overlap_mode, overlap_tree=self.overlap_tree,
                 kf_x_subsamp=self.kf_x_subsamp, keyframe_overlap_thr=self.keyframe_overlap_thr,
                 min_conf_keyframe=self.min_conf_keyframe, overlap_percentile=self.overlap_percentile,
                 to_orig_focal=to_orig_focal)
-            self.all_timestamps.append(fid)
-            self.all_poses.append(pred['slam_c2w'])
-            self.all_confs.append(torch.tensor(pred['slam_record']['conf_mean']))
-            if iskeyframe:
+            if out[-1]:
                 self.memory = newmem
                 kept = True
-                self.keyframes.append(fid)
-                if self.overlap_tree is not None:
-                    self.overlap_tree.add_pts(selpts3d, cam_center=cam_center)
-                    _index_ready(self.overlap_tree, self.device)
-                if self.keep_memory:
-                    self.keyframe_pointmaps.append([pts3d.cpu(), colors.cpu(), conf.cpu()])
+            ret = self._record_frame(view, pred, fid, out)
         if not kept:
             _release_tail(self.memory)        # the update of a frame that is not a keyframe is dropped
-        return pts3d.cpu().numpy(), colors.cpu().numpy(), depth, conf, focal, w2c, HW, iskeyframe
+        return ret
+
+    def _record_frame(self, view, pred, fid, out):
+        """Host bookkeeping of a frame once its record is known (out = the agent's update tuple; the caller updates the
+        memory): its timestamp, pose and confidence; on a keyframe its id, its confident points in the searcher and, with
+        keep_memory, its point map.  -> what __call__ returns for the frame."""
+        selpts3d, pts3d, colors, depth, conf, focal, w2c, cam_center, iskeyframe = out
+        self.all_timestamps.append(fid)
+        self.all_poses.append(pred['slam_c2w'])
+        self.all_confs.append(torch.tensor(pred['slam_record']['conf_mean']))
+        if iskeyframe:
+            self.keyframes.append(fid)
+            if self.overlap_tree is not None:
+                self.overlap_tree.add_pts(selpts3d, cam_center=cam_center)
+                _index_ready(self.overlap_tree, self.device)
+            if self.keep_memory:
+                self.keyframe_pointmaps.append([pts3d.cpu(), colors.cpu(), conf.cpu()])
+        return pts3d.cpu().numpy(), colors.cpu().numpy(), depth, conf, focal, w2c, view['true_shape'][0], iskeyframe

@@ -9,9 +9,11 @@ initialisation re-runs (`num_init_frames`, after a fresh start or a loaded memor
 rows (memory_mode 'kv'), and its preprocessed shape is the batch's shape (the shape most frames of the step share).  The
 batch then costs one encoder call over its frames, one decoder call in which each frame attends only to its own
 session's memory (MUSt3R.update_tokens with mem_lengths, csrc/model.cu m3r_decoder_forward_ragged), the per-session
-pose, searcher query and keyframe kernels, one m3r_mem_commit that appends the new rows of the sessions whose frame is
-a keyframe, and one wait for all records and returned arrays.  Every other frame runs alone through SLAM_MUSt3R.__call__
-and its resulting memory is copied into its session's slot.
+pose, searcher query and keyframe kernels (MUSt3R_Agent.launch_tail, each into its row of one batch of records), one
+m3r_mem_commit that appends the new rows of the sessions whose frame is a keyframe, and one wait for all records and
+returned arrays (engine/slam.py's _wait_host_copies); then each frame finishes as in SLAM_MUSt3R.__call__
+(MUSt3R_Agent.finish_tail, SLAM_MUSt3R._record_frame).  Every other frame runs alone through SLAM_MUSt3R.__call__ and its
+resulting memory is copied into its session's slot.
 
 Memory: per decoder level one arena [S, cap, 2D] (SessionArena); session s's memory is rows [0, n_s) of slot s.  The
 arena grows geometrically, for all sessions with one copy per level, when a session would overflow.  Each session's
@@ -31,9 +33,10 @@ import torch
 from .. import _lib, ops
 from ..model import get_pointmaps_activation, load_model
 from ..model import common as cm
+from . import slam
 from .images import preproc_frame
-from .inference import _reserve, _sync_host_copies, _to_out, postprocess
-from .slam import SLAM_MUSt3R, _index_ready, mean_focal, prep_imgs
+from .inference import _reserve, _to_out, postprocess
+from .slam import SLAM_MUSt3R
 
 KEYFRAME_OFFSET = ops.SLAM_RECORD.fields["keyframe"][1]        # byte offset of the keyframe flag in a record
 
@@ -109,31 +112,13 @@ def slot_runs(slots: Sequence[int]):
 class _Session(SLAM_MUSt3R):
     """One session: SLAM_MUSt3R on a shared model, its memory kept in slot `slot` of the sessions' arena."""
 
-    def __init__(self, model, slot, res=512, searcher='kdtree-scipy-quadrant_x2', overlap_mode='nn-norm', kf_x_subsamp=4,
-                 keyframe_overlap_thr=.15, min_conf_keyframe=1.5, overlap_percentile=70., rerender=False, fixed_focal=True,
-                 keep_memory=False, load_memory=None, num_agents=1, device='cuda:0', num_init_frames=2):
-        from .slam import MUSt3R_Agent
+    def __init__(self, model, slot, **kwargs):
         self.slot = slot
-        self.agents = [MUSt3R_Agent(fixed_focal) for _ in range(num_agents)]
-        self.num_init_frames = num_init_frames
-        self.res = res
-        self.device = device
-        self.model = model
-        self.searcher = searcher
-        self.kf_x_subsamp = kf_x_subsamp
-        self.keyframe_overlap_thr = keyframe_overlap_thr
-        self.min_conf_keyframe = min_conf_keyframe
-        self.overlap_percentile = overlap_percentile
-        self.overlap_mode = overlap_mode
-        self.rerender = rerender
-        self.keep_memory = keep_memory
-        self.memory_memory = None
-        self.memory_map = None
-        self.memory_data = []
-        self.memory_overlap_tree = None
-        if load_memory is not None:
-            self.load_memory(load_memory)
-        self.reset()
+        self._shared_model = model
+        super().__init__(None, **kwargs)
+
+    def _load_model(self, chkpt, device):
+        return self._shared_model
 
     def runs_alone(self):
         """The frames SLAM_MUSt3R.__call__ handles specially: the first one (no memory) and the initialisation re-runs."""
@@ -260,64 +245,31 @@ class SLAMSessions:
         res, staged = self._decode(batch, prepped)
         index = {sid: i for i, sid in enumerate(batch)}
         recs = torch.empty((len(batch), ops.SLAM_RECORD.itemsize), dtype=torch.uint8, device=dev)
-        tails = []
+        preds, tails = [], []
         for i, sid in enumerate(batch):
             s = self.sessions[sid]
-            img, fid, cam = frames[sid]
-            view, to_orig = prepped[sid]
-            agent = s.agents[cam]
             pred = {k: res[k][i:i + 1] for k in ('pts3d', 'pts3d_local', 'conf')}
-            seq_focal = mean_focal(agent.seq_focals) if agent.fixed_focal else None
-            rec = recs[i:i + 1]
-            ops.slam_pose(pred['pts3d'][0], pred['pts3d_local'][0], pred['conf'][0], seq_focal=seq_focal, rec=rec)
-            c2w = ops.slam_record_c2w(rec)[0]
-            cam_center = c2w[:3, -1]
-            sub_s = s.kf_x_subsamp or 1
-            sub = pred['pts3d'][0, 0, ::sub_s, ::sub_s].reshape(-1, 3)
-            conf = pred['conf'][0, 0]
-            dists = None
-            if ops.overlap_mode_id(s.overlap_mode) <= 1:
-                dists = s.overlap_tree.query(sub, cam_center=cam_center).float().contiguous()
-            ops.slam_keyframe(dists, conf, pred['pts3d_local'][0, 0], rec, subsamp=sub_s, mode=s.overlap_mode,
-                              percentile=s.overlap_percentile, thr=s.keyframe_overlap_thr,
-                              min_conf_keyframe=s.min_conf_keyframe, is_first=False)
-            cols = prep_imgs(view['img'], img_mean=agent.img_mean, img_std=agent.img_std)[None]
-            host = [_to_out(t, 'cpu') for t in (pred['pts3d'][0, 0], cols)]
-            tails.append((s, fid, cam, view, to_orig, agent, pred, c2w, cam_center, sub, conf, host))
+            tails.append(s.agents[frames[sid][2]].launch_tail(
+                prepped[sid][0], pred, False, overlap_mode=s.overlap_mode, overlap_tree=s.overlap_tree,
+                kf_x_subsamp=s.kf_x_subsamp, keyframe_overlap_thr=s.keyframe_overlap_thr,
+                min_conf_keyframe=s.min_conf_keyframe, overlap_percentile=s.overlap_percentile, rec=recs[i:i + 1]))
+            preds.append(pred)
         self._commit(staged, recs, index)
         host_recs = _to_out(recs, 'cpu')
-        _wait_step()
+        slam._wait_host_copies()
         records = host_recs.numpy().view(ops.SLAM_RECORD)[:, 0]
         new_rows = {sid: t for members, tok in staged for sid, t in zip(members, [tok] * len(members))}
         out = {}
-        for i, (s, fid, cam, view, to_orig, agent, pred, c2w, cam_center, sub, conf, host) in enumerate(tails):
-            sid = batch[i]
-            r = records[i]
-            iskeyframe = bool(r['keyframe'])
-            sub_s = s.kf_x_subsamp or 1
-            msk = conf[::sub_s, ::sub_s].reshape(-1) > s.min_conf_keyframe
-            pts = sub[torch.argsort((~msk).to(torch.uint8), stable=True)[:int(r['n_conf'])]]
-            pred['overlap_score'], pred['slam_record'], pred['slam_c2w'] = float(r['score']), r, c2w
-            agent.seq_focals['f'].append(np.float32(r['focal']))
-            agent.seq_focals['to_orig'].append(to_orig)
-            agent.seq_focals['conf'].append(np.float32(r['conf_mean']) - 1.)
-            focal = mean_focal(agent.seq_focals) if agent.fixed_focal else agent.seq_focals['f'][-1]
-            w2c = recs[i, 64:128].view(torch.float32).view(4, 4)
+        for i, sid in enumerate(batch):
+            s = self.sessions[sid]
+            _, fid, cam = frames[sid]
+            view, to_orig = prepped[sid]
+            frame_out = s.agents[cam].finish_tail(preds[i], tails[i], records[i], to_orig)
             if s.rerender:
                 s.all_images.append(view)
-            s.all_timestamps.append(fid)
-            s.all_poses.append(c2w)
-            s.all_confs.append(torch.tensor(r['conf_mean']))
-            if iskeyframe:
+            if frame_out[-1]:
                 self._append(s, new_rows[sid][0].shape[1])
-                s.keyframes.append(fid)
-                if s.overlap_tree is not None:
-                    s.overlap_tree.add_pts(pts, cam_center=cam_center)
-                    _index_ready(s.overlap_tree, s.device)
-                if s.keep_memory:
-                    s.keyframe_pointmaps.append([host[0], host[1], conf.cpu()])
-            depth = pred['pts3d_local'][0, 0, ..., -1]
-            out[sid] = (host[0].numpy(), host[1].numpy(), depth, conf, focal, w2c, view['true_shape'][0], iskeyframe)
+            out[sid] = s._record_frame(view, preds[i], fid, frame_out)
         return out
 
     def _append(self, s, n_new):
@@ -327,8 +279,3 @@ class SLAMSessions:
         self.arena.lengths[s.slot] = n
         labels = torch.cat([labels, torch.full((1, n_new), nimgs, dtype=labels.dtype, device=labels.device)], 1)
         s.memory = (self.arena.views(s.slot), labels, nimgs + 1, nimgs + 1, n)
-
-
-def _wait_step():
-    """The one wait of a batched step: every session's record and returned arrays are on the host after it."""
-    _sync_host_copies()

@@ -106,6 +106,12 @@ def parse_args(argv=None):
             parser.error(f"--input {inp}: video files are not supported (they need cv2); give a folder of frames")
         if not os.path.isdir(inp):
             parser.error(f"--input {inp}: no such folder")
+    check_device_and_skip(parser, args)
+    return args
+
+
+def check_device_and_skip(parser, args):
+    """Reject through `parser` a --device that is not a CUDA device and a --skip_every below 1."""
     try:
         dev = torch.device(args.device)
     except RuntimeError:
@@ -114,7 +120,27 @@ def parse_args(argv=None):
         parser.error(f"--device {args.device}: must3r_b200 runs on CUDA devices only")
     if args.skip_every < 1:
         parser.error("--skip_every must be at least 1")
-    return args
+
+
+def resolve_device(name):
+    """The CUDA device `name` names, with the current device's index when it has none."""
+    device = torch.device(name)
+    if device.index is None:
+        device = torch.device('cuda', torch.cuda.current_device())
+    return device
+
+
+def write_poses(model, output, filtered, **tolog):
+    """model.write_all_poses into OUTPUT/all_poses.npz, or when `filtered` the Laplacian-smoothed poses into
+    OUTPUT/all_poses{mode}_{steps}-steps_{alpha}-alpha.npz -> the file's path."""
+    if not filtered:
+        outfile = os.path.join(output, 'all_poses.npz')
+        model.write_all_poses(outfile, **tolog)
+    else:
+        outfile = os.path.join(output, f"all_poses{FILTERING_MODE}_{FILTERING_STEPS}-steps_{FILTERING_ALPHA}-alpha.npz")
+        model.write_all_poses(outfile, filtering_mode=FILTERING_MODE, filtering_steps=FILTERING_STEPS,
+                              filtering_alpha=FILTERING_ALPHA, **tolog)
+    return outfile
 
 
 def memory_path(output, load_memory=None):
@@ -165,9 +191,7 @@ def main(argv=None, read_ahead=True):
     decodes every frame before the clock starts, as the reference does; it exists for tools/bench_slam_cli.py's
     comparison, and no command-line option selects it."""
     args = parse_args(argv)
-    device = torch.device(args.device)
-    if device.index is None:
-        device = torch.device('cuda', torch.cuda.current_device())
+    device = resolve_device(args.device)
     model = SLAM_MUSt3R(chkpt=args.chkpt,
                         res=args.res,
                         kf_x_subsamp=args.subsamp,
@@ -206,15 +230,7 @@ def main(argv=None, read_ahead=True):
         gpumem = torch.cuda.max_memory_allocated(device) / MB
     print(f"Done @{fps}fps on average using {gpumem}MB GPU Memory")
     print(f"{len(model.keyframes)} keyframes: {model.keyframes}")
-    tolog = {'fps': fps, 'gpumem': gpumem, 'imgHWs': imgHWs}
-
-    if not args.filter:
-        outfile = os.path.join(args.output, 'all_poses.npz')
-        model.write_all_poses(outfile, **tolog)
-    else:
-        outfile = os.path.join(args.output, f"all_poses{FILTERING_MODE}_{FILTERING_STEPS}-steps_{FILTERING_ALPHA}-alpha.npz")
-        model.write_all_poses(outfile, filtering_mode=FILTERING_MODE, filtering_steps=FILTERING_STEPS,
-                              filtering_alpha=FILTERING_ALPHA, **tolog)
+    outfile = write_poses(model, args.output, args.filter, fps=fps, gpumem=gpumem, imgHWs=imgHWs)
     outname = memory_path(args.output, args.load_memory)
     print(f"Dumping memory as {outname}")
     model.save_memory(outname)

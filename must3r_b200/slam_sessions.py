@@ -47,23 +47,14 @@ def parse_args(argv=None):
     for d in args.sessions:
         if not os.path.isdir(d):
             parser.error(f"--sessions {d}: no such folder")
-    try:
-        dev = torch.device(args.device)
-    except RuntimeError:
-        parser.error(f"--device {args.device}: not a device")
-    if dev.type != 'cuda':
-        parser.error(f"--device {args.device}: must3r_b200 runs on CUDA devices only")
-    if args.skip_every < 1:
-        parser.error("--skip_every must be at least 1")
+    single.check_device_and_skip(parser, args)
     return args
 
 
 def main(argv=None):
     """-> the poses file of every session."""
     args = parse_args(argv)
-    device = torch.device(args.device)
-    if device.index is None:
-        device = torch.device('cuda', torch.cuda.current_device())
+    device = single.resolve_device(args.device)
     S = len(args.sessions)
     model = SLAMSessions(args.chkpt, S, device=str(device), res=args.res, kf_x_subsamp=args.subsamp,
                          searcher=args.searcher, overlap_mode=args.overlap_mode,
@@ -109,17 +100,8 @@ def main(argv=None):
     outfiles = []
     for i, s in enumerate(model.sessions):
         print(f"session {i}: {len(s.keyframes)} keyframes: {s.keyframes}")
-        tolog = {'fps': fps, 'gpumem': gpumem, 'imgHWs': imgHWs[i]}
-        if not args.filter:
-            outfile = os.path.join(outdirs[i], 'all_poses.npz')
-            s.write_all_poses(outfile, **tolog)
-        else:
-            outfile = os.path.join(outdirs[i], f"all_poses{single.FILTERING_MODE}_{single.FILTERING_STEPS}-steps_"
-                                               f"{single.FILTERING_ALPHA}-alpha.npz")
-            s.write_all_poses(outfile, filtering_mode=single.FILTERING_MODE, filtering_steps=single.FILTERING_STEPS,
-                              filtering_alpha=single.FILTERING_ALPHA, **tolog)
+        outfiles.append(single.write_poses(s, outdirs[i], args.filter, fps=fps, gpumem=gpumem, imgHWs=imgHWs[i]))
         s.save_memory(os.path.join(outdirs[i], "memory.pkl"))
-        outfiles.append(outfile)
     return outfiles
 
 

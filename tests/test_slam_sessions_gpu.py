@@ -225,12 +225,12 @@ def test_saved_session_memory_continues_like_the_live_memory(three, chkpt):
     assert b1.keyframes == b2.keyframes
 
 
-def test_step_without_keyframe_syncs_only_at_its_one_wait(chkpt, monkeypatch, g):
+def test_step_without_keyframe_syncs_only_at_the_shared_wait(chkpt, monkeypatch, g):
     frames = mk.frames()
     ss = SLAMSessions(chkpt, 2, device="cuda:0", **E2E)
     _stepped(ss, [frames[:4], frames[:4]])
     waits = []
-    dec, wait = SLAMSessions._decode, slam_sessions._wait_step
+    dec, wait = SLAMSessions._decode, slam._wait_host_copies
 
     def decode_then_strict(self, *a, **k):
         out = dec(self, *a, **k)
@@ -244,7 +244,7 @@ def test_step_without_keyframe_syncs_only_at_its_one_wait(chkpt, monkeypatch, g)
         torch.cuda.set_sync_debug_mode("error")
 
     monkeypatch.setattr(SLAMSessions, "_decode", decode_then_strict)
-    monkeypatch.setattr(slam_sessions, "_wait_step", named_wait)
+    monkeypatch.setattr(slam, "_wait_host_copies", named_wait)
     try:
         out = ss.step({0: (frames[4], 4, 0), 1: (frames[4], 4, 0)})
     finally:

@@ -42,7 +42,7 @@ def run_batched(chkpt, seqs, warmup, res):
     ss = ssm.SLAMSessions(chkpt, len(seqs), device="cuda:0", res=res)
     enc = ss.model[0]
     marks = []
-    fwd, dec, wait = enc.forward, ssm.SLAMSessions._decode, ssm._wait_step
+    fwd, dec, wait = enc.forward, ssm.SLAMSessions._decode, slam._wait_host_copies
 
     def ev():
         e = torch.cuda.Event(enable_timing=True)
@@ -61,10 +61,11 @@ def run_batched(chkpt, seqs, warmup, res):
         return out
 
     def timed_wait():
-        marks[-1].append(ev())
+        if len(marks[-1]) == 3:                 # a batched step's wait, not that of a frame run alone (no decode mark)
+            marks[-1].append(ev())
         wait()
 
-    enc.forward, ssm.SLAMSessions._decode, ssm._wait_step = timed_encoder, timed_decode, timed_wait
+    enc.forward, ssm.SLAMSessions._decode, slam._wait_host_copies = timed_encoder, timed_decode, timed_wait
     try:
         n = len(seqs[0])
         for k in range(warmup):
@@ -78,7 +79,7 @@ def run_batched(chkpt, seqs, warmup, res):
         wall = time.perf_counter() - t0
     finally:
         del enc.forward
-        ssm.SLAMSessions._decode, ssm._wait_step = dec, wait
+        ssm.SLAMSessions._decode, slam._wait_host_copies = dec, wait
     full = [m for m in marks if len(m) == 4]
     split = {name: round(float(np.median([m[i].elapsed_time(m[i + 1]) for m in full])), 3) if full else None
              for i, name in enumerate(("encoder_ms", "decoder_ms", "tail_ms"))}
