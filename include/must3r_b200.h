@@ -8,7 +8,8 @@
  *
  * Each function names the reference interface it replaces (paths relative to the reference repo).
  * 16-bit operands are fp16 (is_bf16 = 0) or bf16 (is_bf16 = 1); accumulation, LayerNorm, softmax and the
- * residual stream are fp32.
+ * residual stream are fp32.  The *_e4m3 entry points add float8 e4m3 operands for the GEMMs whose A operand is an
+ * affine-free LayerNorm output (the other operands stay bf16); they leave every existing struct and entry point as it was.
  */
 #ifndef MUST3R_B200_H
 #define MUST3R_B200_H
@@ -30,6 +31,7 @@ extern "C" {
 /* out_dtype */
 #define M3R_OUT_F32 0
 #define M3R_OUT_16 1
+#define M3R_OUT_E4M3 2   /* float8 e4m3 bytes (round to nearest even; finite values beyond +-448 saturate to +-448) */
 /* activation */
 #define M3R_ACT_NONE 0
 #define M3R_ACT_GELU 1
@@ -105,6 +107,23 @@ typedef struct {
 
 int m3r_gemm(const m3r_gemm_args* args, void* stream);
 
+/* e4m3 options of a GEMM (m3r_gemm_e4m3 / m3r_gemm_grouped_e4m3; a NULL pointer = m3r_gemm / m3r_gemm_grouped):
+ * a_e4m3 = 1: A [M,K] and W [N,K] are float8 e4m3 (1 byte per element; lda / ldw multiples of 16, K % 128 == 0, N % 64 ==
+ *   0), is_bf16 must be 1 (16-bit outputs are bf16), and accumulator column n is multiplied by w_scale[n] before bias,
+ *   RoPE, GELU, residual, norm_out and the stores (grouped form: w_scale is indexed by the row of the stacked W, like W).
+ *   w_scale is required (8-byte aligned).  W = round_e4m3(W_true / w_scale) row by row.  Not combinable with norm_out
+ *   (the GEMMs that emit a LayerNorm have unbounded 16-bit A operands).
+ * norm_e4m3 = 1: norm_out rows are written as e4m3 (ldn in bytes, a multiple of 16; M3R_OUT_E4M3).  The normalised row
+ *   (x - mean) * rstd of D values has |y| <= sqrt(D - 1) (<= 32 for D <= 1025), far inside e4m3's range, so no scale
+ *   is needed for it. */
+typedef struct {
+  int32_t a_e4m3;
+  const float* w_scale;
+  int32_t norm_e4m3;
+} m3r_gemm_e4m3_args;
+
+int m3r_gemm_e4m3(const m3r_gemm_args* args, const m3r_gemm_e4m3_args* e8, void* stream);
+
 /* Grouped form: `groups` problems of identical shape [args->M, args->N, args->K] in one launch.  A = [groups*M, K]
  * (group g = rows [g*M, (g+1)*M)), W rows [g*w_group_rows, +N), bias + g*bias_group; args->out / peer_out are ignored,
  * group g writes out[g] (and peer_out[g*M3R_MAX_PEERS + r], r < args->n_peer_out) with args' ldc / row remap.
@@ -121,6 +140,7 @@ typedef struct {
 } m3r_gemm_group;
 
 int m3r_gemm_grouped(const m3r_gemm_args* args, const m3r_gemm_group* grp, void* stream);
+int m3r_gemm_grouped_e4m3(const m3r_gemm_args* args, const m3r_gemm_group* grp, const m3r_gemm_e4m3_args* e8, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
  * LayerNorm over the last dim of fp32 rows (optionally of x + add), output 16-bit (GEMM operand) or fp32.
@@ -139,6 +159,9 @@ int m3r_layernorm(const float* x, int64_t ldx, const float* add, int64_t ldadd, 
  * normalised rows itself (m3r_gemm_args.norm_out: multi-wave problems). */
 int m3r_normalize16(const float* x, int64_t ldx, const float* add, int64_t ldadd, int32_t add_rows, int32_t add_period,
                     float eps, int32_t M, int32_t D, void* out16, int64_t ldo, int32_t is_bf16, void* stream);
+/* The same rows written as e4m3 bytes (M3R_OUT_E4M3; ldo in bytes, a multiple of 4): the A operand of an e4m3 GEMM. */
+int m3r_normalize8(const float* x, int64_t ldx, const float* add, int64_t ldadd, int32_t add_rows, int32_t add_period,
+                   float eps, int32_t M, int32_t D, void* out8, int64_t ldo, void* stream);
 
 /* fp32 -> 16-bit cast of [M,D] rows (encoder features entering the decoder projector, decoder.py:274). */
 int m3r_cast16(const float* x, int64_t ldx, int32_t M, int32_t D, void* out, int64_t ldo, int32_t is_bf16,
@@ -368,6 +391,18 @@ int64_t m3r_encoder_workspace_bytes(const m3r_encoder_weights* w, int32_t V, int
 int m3r_encoder_forward(const m3r_encoder_weights* w, const float* img, int32_t V, int32_t H, int32_t W,
                         const int64_t* pos, float* out_x, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* FP8 encoder (same workspace): w->is_bf16 = 1 and, per block, qkv_w / fc1_w are e4m3 [3D,D] / [4D,D] with norm1 / norm2
+ * folded in (W * diag(gamma), b + W beta, then quantised row by row; norm1_w .. norm2_b unused); blocks8[l] holds their
+ * per-row scales.  Each LayerNorm before qkv / fc1 becomes an affine-free m3r_normalize8; patch embedding, proj, fc2,
+ * attention and the residual stream run as in bf16. */
+typedef struct {
+  const float* qkv_s;     /* [3D] */
+  const float* fc1_s;     /* [4D] */
+} m3r_enc_block_e4m3;
+int m3r_encoder_forward_e4m3(const m3r_encoder_weights* w, const m3r_enc_block_e4m3* blocks8, const float* img, int32_t V,
+                             int32_t H, int32_t W, const int64_t* pos, float* out_x, void* workspace,
+                             int64_t workspace_bytes, void* stream);
+
 /* CachedDecoderBlock (must3r/model/blocks/layers.py:57-99).  Every LayerNorm of the block is applied WITHOUT its affine
  * (by the epilogue of the GEMM that produced the rows, m3r_gemm_args.norm_out, or by m3r_normalize16); the affine lives in the
  * consuming Linear: W' = W * diag(gamma), b' = b + W beta (exact in real arithmetic; rounded to 16 bits once, like W).
@@ -489,6 +524,22 @@ int m3r_decoder_forward(const m3r_decoder_weights* w, const m3r_decoder_call* ca
  * workspace is m3r_decoder_workspace_bytes(w, call). */
 int m3r_decoder_forward_ragged(const m3r_decoder_weights* w, const m3r_decoder_call* call, const int32_t* nm_scene,
                                void* workspace, int64_t workspace_bytes, void* stream);
+
+/* FP8 decoder: w->is_bf16 = 1, and the GEMMs fed by an affine-free LayerNorm take e4m3 operands: a_w (qkv | projk;projv,
+ * [depth, 5D, D] e4m3, one byte per element), q_w, fc1_w and (feedback) fb1_w hold e4m3 weights with per-row scales in w8.
+ * Everything else (proj, cproj, fc2, embed, head, the K|V memory, attention) stays bf16.  nm_scene = NULL runs
+ * m3r_decoder_forward, otherwise m3r_decoder_forward_ragged; same workspace. */
+typedef struct {
+  const float* a_s;       /* [5D]; blocks[l].a_s == blocks[0].a_s + l*5D for the grouped memory append */
+  const float* q_s;       /* [D] */
+  const float* fc1_s;     /* [4D] */
+} m3r_dec_block_e4m3;
+typedef struct {
+  const m3r_dec_block_e4m3* blocks;  /* host array [depth] */
+  const float* fb1_s;                /* [4D] (single_mlp) or [D] (single_linear); NULL without feedback */
+} m3r_decoder_e4m3;
+int m3r_decoder_forward_e4m3(const m3r_decoder_weights* w, const m3r_decoder_e4m3* w8, const m3r_decoder_call* call,
+                             const int32_t* nm_scene, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* Keyframe commit of several SLAM sessions in one launch: for each scene b < B whose flag keep[b * keep_stride] (int32,
  * device; e.g. the keyframe field of its m3r_slam_record) is non-zero, copy rows [0, Nt) of staged[l] + b * Nt * width

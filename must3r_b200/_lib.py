@@ -34,6 +34,10 @@ class GemmArgs(C.Structure):
     ]
 
 
+class GemmE4M3Args(C.Structure):
+    _fields_ = [("a_e4m3", C.c_int32), ("w_scale", C.c_void_p), ("norm_e4m3", C.c_int32)]
+
+
 class GemmGroup(C.Structure):
     _fields_ = [("groups", C.c_int32), ("w_group_rows", C.c_int64), ("bias_group", C.c_int64),
                 ("out", C.c_void_p * 16), ("peer_out", C.c_void_p * (16 * 8)), ("max_ctas", C.c_int32)]
@@ -64,8 +68,12 @@ SIGNATURES = {
     "m3r_prof_read": (C.c_int, [C.POINTER(C.c_double)]),
     "m3r_gemm": (C.c_int, [C.POINTER(GemmArgs), C.c_void_p]),
     "m3r_gemm_grouped": (C.c_int, [C.POINTER(GemmArgs), C.POINTER(GemmGroup), C.c_void_p]),
+    "m3r_gemm_e4m3": (C.c_int, [C.POINTER(GemmArgs), C.POINTER(GemmE4M3Args), C.c_void_p]),
+    "m3r_gemm_grouped_e4m3": (C.c_int, [C.POINTER(GemmArgs), C.POINTER(GemmGroup), C.POINTER(GemmE4M3Args), C.c_void_p]),
     "m3r_normalize16": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_float, C.c_int32, C.c_int32,
                                   C.c_void_p, C.c_int64, C.c_int32, C.c_void_p]),
+    "m3r_normalize8": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_float, C.c_int32, C.c_int32,
+                                 C.c_void_p, C.c_int64, C.c_void_p]),
     "m3r_layernorm": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_float,
                                 C.c_int32, C.c_int32, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p]),
     "m3r_cast16": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p]),

@@ -84,8 +84,10 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const void* __restrict__
         const float4 g = PRE ? gv[PRE ? i : 0] : __ldg(g4 + idx), b = PRE ? bv[PRE ? i : 0] : __ldg(b4 + idx);
         y.x = y.x * g.x + b.x; y.y = y.y * g.y + b.y; y.z = y.z * g.z + b.z; y.w = y.w * g.w + b.w;
       }
-      if (out_dtype == 0) {
+      if (out_dtype == M3R_OUT_F32) {
         reinterpret_cast<float4*>(reinterpret_cast<float*>(out) + (long long)row * ldo)[idx] = y;
+      } else if (out_dtype == M3R_OUT_E4M3) {
+        reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(out) + (long long)row * ldo)[idx] = pack_e4m3x4(y.x, y.y, y.z, y.w);
       } else {
         uint2 w;
         w.x = pack16(y.x, y.y, is_bf16);
@@ -341,11 +343,12 @@ static int layernorm_impl(const float* x, int64_t ldx, const float* add, int64_t
   if (D % 4 || D > 2048 || ldx % 4 || (add && ldadd % 4) || ldo % 4) return set_error("layernorm: D=%d must be a multiple of 4, <= 2048, 16B-aligned rows", D);
   if (misaligned(x, 16) || misaligned(add, 16) || misaligned(gamma, 16) || misaligned(beta, 16))
     return set_error("layernorm: x, add, gamma and beta must be 16-byte aligned (float4 loads)");
-  if (misaligned(out, out_dtype == M3R_OUT_F32 ? 16 : 8)) return set_error("layernorm: out must be %d-byte aligned", out_dtype == M3R_OUT_F32 ? 16 : 8);
+  const int out_align = out_dtype == M3R_OUT_F32 ? 16 : out_dtype == M3R_OUT_E4M3 ? 4 : 8;
+  if (misaligned(out, out_align)) return set_error("layernorm: out must be %d-byte aligned", out_align);
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   const int wpb = M <= 4096 ? 4 : 8;          // small row counts: more, smaller blocks cover more SMs
   const int grid = (M + wpb - 1) / wpb;
-  ProfScope prof(PROF_LN, 0.0, (double)M * D * (4.0 + (add ? 4.0 : 0.0) + (out_dtype ? 2.0 : 4.0)), s);
+  ProfScope prof(PROF_LN, 0.0, (double)M * D * (4.0 + (add ? 4.0 : 0.0) + (out_dtype == M3R_OUT_E4M3 ? 1.0 : out_dtype ? 2.0 : 4.0)), s);
   if (D <= 1024 && M <= 4096)
     launch_pdl(layernorm_kernel<8, false, true>, dim3(grid), dim3(wpb * 32), 0, s, (const void*)x, (long long)ldx, add, (long long)ldadd, gamma, beta, eps, (int)M, (int)D, out, (long long)ldo, (int)out_dtype, (int)is_bf16, add_rows, add_period);
   else if (D <= 1024)
@@ -366,6 +369,14 @@ extern "C" int m3r_normalize16(const float* x, int64_t ldx, const float* add, in
                                float eps, int32_t M, int32_t D, void* out16, int64_t ldo, int32_t is_bf16, void* stream) {
   if (add && (add_rows < 0 || add_period <= 0)) return set_error("normalize16: bad add_rows / add_period");
   return layernorm_impl(x, ldx, add, ldadd, add ? add_rows : 0, add ? add_period : 1, nullptr, nullptr, eps, M, D, out16, ldo, M3R_OUT_16, is_bf16, stream);
+}
+
+// Affine-free rows as e4m3: |(x - mean) * rstd| <= sqrt(D - 1) for a row of D values (equality when one value differs
+// from all the others), i.e. <= 45 for D <= 2048, well inside e4m3's +-448; the A operand of an e4m3 GEMM needs no scale.
+extern "C" int m3r_normalize8(const float* x, int64_t ldx, const float* add, int64_t ldadd, int32_t add_rows, int32_t add_period,
+                              float eps, int32_t M, int32_t D, void* out8, int64_t ldo, void* stream) {
+  if (add && (add_rows < 0 || add_period <= 0)) return set_error("normalize8: bad add_rows / add_period");
+  return layernorm_impl(x, ldx, add, ldadd, add ? add_rows : 0, add ? add_period : 1, nullptr, nullptr, eps, M, D, out8, ldo, M3R_OUT_E4M3, 0, stream);
 }
 
 extern "C" int m3r_layernorm16(const void* x16, int64_t ldx, const float* gamma, const float* beta, float eps, int32_t M,

@@ -52,7 +52,8 @@ struct ProfScope {
 
 // 2-D TMA descriptor over a row-major 16-bit (or, with fp32, 32-bit float) matrix: inner extent `cols` (contiguous),
 // outer extent `rows`, leading dimension `ld` elements, box = {box_cols, box_rows}, 128-byte swizzle, OOB reads return
-// zeros and OOB writes are dropped.
+// zeros and OOB writes are dropped.  is_bf16 == TMAP_E4M3: 1-byte e4m3 elements.
+constexpr int TMAP_E4M3 = 2;
 int make_tmap_2d(CUtensorMap* out, const void* base, int is_bf16, uint64_t cols, uint64_t rows, uint64_t ld,
                  uint32_t box_cols, uint32_t box_rows, bool fp32 = false);
 

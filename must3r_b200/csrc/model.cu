@@ -34,7 +34,8 @@ static int gemm(const void* A, int64_t lda, const void* W, int64_t ldw, int M, i
                 const float* bias, int act, const float* residual, int64_t ldr, void* out, int64_t ldc, int out_dtype,
                 void* stream, const float* rope_tab = nullptr, int rope_cols = 0, int rope_period = 0,
                 const float* rowbias = nullptr, int rb_period = 1, int rb_first = 0, int rows_per_batch = 0,
-                int64_t batch_stride_rows = 0, int n_peer_out = 0, void* const* peer_out = nullptr) {
+                int64_t batch_stride_rows = 0, int n_peer_out = 0, void* const* peer_out = nullptr,
+                const float* w_scale = nullptr) {
   m3r_gemm_args a = {};
   a.n_peer_out = n_peer_out;
   a.w_static = 1;                  // every GEMM of the model multiplies by checkpoint weights
@@ -45,7 +46,17 @@ static int gemm(const void* A, int64_t lda, const void* W, int64_t ldw, int M, i
   a.rope_tab = rope_tab; a.rope_cols = rope_cols; a.rope_period = rope_period;
   a.out = out; a.ldc = ldc; a.out_dtype = out_dtype;
   a.rows_per_batch = rows_per_batch; a.batch_stride_rows = batch_stride_rows;
-  return m3r_gemm(&a, stream);
+  if (!w_scale) return m3r_gemm(&a, stream);
+  m3r_gemm_e4m3_args e8 = {};                // A and W are e4m3, W row n scaled by w_scale[n]
+  e8.a_e4m3 = 1; e8.w_scale = w_scale;
+  return m3r_gemm_e4m3(&a, &e8, stream);
+}
+
+// The affine-free LayerNorm of the rows feeding the next GEMM: e4m3 bytes when that GEMM takes e4m3 operands
+static int normalize(bool e4m3, const float* x, const float* add, int add_rows, int add_period, float eps, int M, int D,
+                     void* out, int bf, void* stream) {
+  if (e4m3) return m3r_normalize8(x, D, add, D, add_rows, add_period, eps, M, D, out, D, stream);
+  return m3r_normalize16(x, D, add, D, add_rows, add_period, eps, M, D, out, D, bf, stream);
 }
 
 struct EncWs { uint16_t *cols16, *h16, *qkv16, *att16, *mlp16; float *x, *rope; };
@@ -72,9 +83,11 @@ extern "C" int64_t m3r_encoder_workspace_bytes(const m3r_encoder_weights* w, int
   return enc_layout(w, V, H, W, nullptr, 0, &ws);
 }
 
-extern "C" int m3r_encoder_forward(const m3r_encoder_weights* w, const float* img, int32_t V, int32_t H, int32_t W,
-                                   const int64_t* pos, float* out_x, void* workspace, int64_t workspace_bytes,
-                                   void* stream) {
+namespace m3r {
+
+// b8 != null: qkv and fc1 take e4m3 operands (their LayerNorms folded into the weights, the rows normalised to e4m3)
+static int encoder_forward(const m3r_encoder_weights* w, const m3r_enc_block_e4m3* b8, const float* img, int32_t V, int32_t H,
+                           int32_t W, const int64_t* pos, float* out_x, void* workspace, int64_t workspace_bytes, void* stream) {
   if (!w || !img || !pos || !out_x || !workspace) return set_error("encoder_forward: null pointer");
   if (H % 16 || W % 16) return set_error("Input image size (%d,%d) is not a multiple of patch size 16", H, W);  // patch_embed.py:22-23
   if (w->embed_dim != w->num_heads * 64) return set_error("encoder_forward: head_dim must be 64");
@@ -90,23 +103,43 @@ extern "C" int m3r_encoder_forward(const m3r_encoder_weights* w, const float* im
   M3R_TRY(gemm(ws.cols16, 768, w->patch_w, 768, M, D, 768, bf, w->patch_b, 0, nullptr, 0, ws.x, D, M3R_OUT_F32, stream));
   for (int l = 0; l < w->depth; ++l) {
     const m3r_enc_block& b = w->blocks[l];
-    M3R_TRY(m3r_layernorm(ws.x, D, nullptr, 0, b.norm1_w, b.norm1_b, w->ln_eps, M, D, ws.h16, D, M3R_OUT_16, bf, stream));
+    if (b8) M3R_TRY(m3r_normalize8(ws.x, D, nullptr, 0, 0, 1, w->ln_eps, M, D, ws.h16, D, stream));
+    else M3R_TRY(m3r_layernorm(ws.x, D, nullptr, 0, b.norm1_w, b.norm1_b, w->ln_eps, M, D, ws.h16, D, M3R_OUT_16, bf, stream));
     M3R_TRY(gemm(ws.h16, D, b.qkv_w, D, M, 3 * D, D, bf, b.qkv_b, 0, nullptr, 0, ws.qkv16, 3 * D, M3R_OUT_16, stream,
-                 ws.rope, 2 * D, N));
+                 ws.rope, 2 * D, N, nullptr, 1, 0, 0, 0, 0, nullptr, b8 ? b8[l].qkv_s : nullptr));
     m3r_attn_args at = {};
     at.Q = ws.qkv16; at.ldq = 3 * D;
     at.K0 = ws.qkv16 + D; at.V0 = ws.qkv16 + 2 * D; at.ldk0 = 3 * D; at.kv_bstride0 = N; at.Nk0 = N;
     at.O = ws.att16; at.ldo = D; at.B = V; at.H = Hh; at.Nq = N; at.kv_group = 1; at.is_bf16 = bf; at.scale = 0.125f;
     M3R_TRY(m3r_attention(&at, stream));
     M3R_TRY(gemm(ws.att16, D, b.proj_w, D, M, D, D, bf, b.proj_b, 0, ws.x, D, ws.x, D, M3R_OUT_F32, stream));
-    M3R_TRY(m3r_layernorm(ws.x, D, nullptr, 0, b.norm2_w, b.norm2_b, w->ln_eps, M, D, ws.h16, D, M3R_OUT_16, bf, stream));
+    if (b8) M3R_TRY(m3r_normalize8(ws.x, D, nullptr, 0, 0, 1, w->ln_eps, M, D, ws.h16, D, stream));
+    else M3R_TRY(m3r_layernorm(ws.x, D, nullptr, 0, b.norm2_w, b.norm2_b, w->ln_eps, M, D, ws.h16, D, M3R_OUT_16, bf, stream));
     M3R_TRY(gemm(ws.h16, D, b.fc1_w, D, M, w->mlp_hidden, D, bf, b.fc1_b, M3R_ACT_GELU, nullptr, 0, ws.mlp16,
-                 w->mlp_hidden, M3R_OUT_16, stream));
+                 w->mlp_hidden, M3R_OUT_16, stream, nullptr, 0, 0, nullptr, 1, 0, 0, 0, 0, nullptr, b8 ? b8[l].fc1_s : nullptr));
     M3R_TRY(gemm(ws.mlp16, w->mlp_hidden, b.fc2_w, w->mlp_hidden, M, D, w->mlp_hidden, bf, b.fc2_b, 0, ws.x, D, ws.x, D,
                  M3R_OUT_F32, stream));
   }
   M3R_TRY(m3r_layernorm(ws.x, D, nullptr, 0, w->norm_w, w->norm_b, w->ln_eps, M, D, out_x, D, M3R_OUT_F32, 0, stream));
   return 0;
+}
+
+}  // namespace m3r
+
+extern "C" int m3r_encoder_forward(const m3r_encoder_weights* w, const float* img, int32_t V, int32_t H, int32_t W,
+                                   const int64_t* pos, float* out_x, void* workspace, int64_t workspace_bytes,
+                                   void* stream) {
+  return encoder_forward(w, nullptr, img, V, H, W, pos, out_x, workspace, workspace_bytes, stream);
+}
+
+extern "C" int m3r_encoder_forward_e4m3(const m3r_encoder_weights* w, const m3r_enc_block_e4m3* blocks8, const float* img,
+                                        int32_t V, int32_t H, int32_t W, const int64_t* pos, float* out_x, void* workspace,
+                                        int64_t workspace_bytes, void* stream) {
+  if (!blocks8) return set_error("encoder_forward_e4m3: null pointer");
+  if (!w || !w->is_bf16) return set_error("encoder_forward_e4m3: the 16-bit operands of the e4m3 encoder are bf16 (is_bf16 = 1)");
+  for (int l = 0; l < w->depth; ++l)
+    if (!blocks8[l].qkv_s || !blocks8[l].fc1_s) return set_error("encoder_forward_e4m3: block %d has no weight scales", l);
+  return encoder_forward(w, blocks8, img, V, H, W, pos, out_x, workspace, workspace_bytes, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ decoder
@@ -217,9 +250,10 @@ extern "C" int64_t m3r_decoder_workspace_bytes(const m3r_decoder_weights* w, con
 
 namespace m3r {
 
-// nm_scene != null: the ragged update of m3r_decoder_forward_ragged (checked there)
-static int decoder_forward(const m3r_decoder_weights* w, const m3r_decoder_call* c, const int32_t* nm_scene,
-                           void* workspace, int64_t workspace_bytes, void* stream) {
+// nm_scene != null: the ragged update of m3r_decoder_forward_ragged (checked there).  w8 != null: the GEMMs fed by an
+// affine-free LayerNorm (a_w, q_w, fc1_w, fb1_w) take e4m3 operands, and the LayerNorms feeding them write e4m3 rows.
+static int decoder_forward(const m3r_decoder_weights* w, const m3r_decoder_e4m3* w8, const m3r_decoder_call* c,
+                           const int32_t* nm_scene, void* workspace, int64_t workspace_bytes, void* stream) {
   if (!w || !c || !workspace || !c->groups) return set_error("decoder_forward: null pointer");
   if (c->B <= 0 || c->G <= 0) return set_error("decoder_forward: empty call");
   if (w->embed_dim != w->num_heads * 64) return set_error("decoder_forward: head_dim must be 64");
@@ -243,6 +277,14 @@ static int decoder_forward(const m3r_decoder_weights* w, const m3r_decoder_call*
   cudaStream_t cs = reinterpret_cast<cudaStream_t>(stream);
   const int D = w->embed_dim, Hh = w->num_heads, bf = w->is_bf16, B = c->B, G = c->G, Nm = c->Nm;
   const int depth = w->depth;
+  const bool f8 = w8 != nullptr;
+  const int64_t asz = f8 ? 1 : 2;                          // bytes per element of a_w
+  auto a_kv = [&](const m3r_dec_block& b) { return reinterpret_cast<const uint8_t*>(b.a_w) + 3 * D * D * asz; };   // rows [3D, 5D)
+  auto s_of = [&](int l, int which) -> const float* {      // per-row weight scales (null in 16-bit mode)
+    if (!f8) return nullptr;
+    const m3r_dec_block_e4m3& e = w8->blocks[l];
+    return which == 0 ? e.a_s : which == 1 ? e.a_s + 3 * D : which == 2 ? e.q_s : e.fc1_s;
+  };
   const int M = (int)ws.M;
   const int Nt = (int)ws.Nt;
   const int mode = c->mem_mode;
@@ -286,16 +328,19 @@ static int decoder_forward(const m3r_decoder_weights* w, const m3r_decoder_call*
   const int tiles_m = (M + 127) / 128;
   const bool emit = D % 64 == 0 && D <= 768 && tiles_m <= 16 && tiles_m * (D / 64) <= num_sms();
   // residual-stream GEMM: xo = xr + A W^T + b, followed by (or fused with) the normalisation of xo into h16
+  // norm8: the normalised rows feed an e4m3 GEMM
   auto res_gemm = [&](const void* A, int64_t lda, const void* W, int K, const float* bias, const float* xr, float* xo,
-                      const float* rowbias, int rb_period, int rb_first, int Mrows, int64_t row_off) -> int {
+                      const float* rowbias, int rb_period, int rb_first, int Mrows, int64_t row_off, bool norm8) -> int {
     m3r_gemm_args a = {};
     a.A = A; a.lda = lda; a.W = W; a.ldw = K; a.M = Mrows; a.N = D; a.K = K; a.is_bf16 = bf; a.bias = bias;
     a.residual = xr ? xr + row_off * D : nullptr; a.ldr = D; a.out = xo + row_off * D; a.ldc = D; a.out_dtype = M3R_OUT_F32;
     a.rowbias = rowbias; a.rb_period = rb_period; a.rb_first = rb_first; a.w_static = 1;
     if (emit && Mrows == M) { a.norm_out = ws.h16; a.ldn = D; a.norm_eps = w->ln_eps; }
-    M3R_TRY(m3r_gemm(&a, stream));
+    m3r_gemm_e4m3_args e8 = {};
+    e8.norm_e4m3 = norm8 && a.norm_out;
+    M3R_TRY(m3r_gemm_e4m3(&a, &e8, stream));
     if (!(emit && Mrows == M) && row_off + Mrows == M)      // (grouped prologue: normalise once, after the last group)
-      M3R_TRY(m3r_normalize16(xo, D, nullptr, 0, 0, 1, w->ln_eps, M, D, ws.h16, D, bf, stream));
+      M3R_TRY(normalize(norm8, xo, nullptr, 0, 1, w->ln_eps, M, D, ws.h16, bf, stream));
     return 0;
   };
 
@@ -309,7 +354,7 @@ static int decoder_forward(const m3r_decoder_weights* w, const m3r_decoder_call*
     M3R_TRY(m3r_cast16(gr.x_enc, w->enc_dim, Mg, w->enc_dim, ws.enc16 + ws.row0[g] * w->enc_dim, w->enc_dim, bf, stream));
     const int first = (c->is_init && g == 0) ? gr.N : 0;    // rows of view 0 of every scene get no embed at init
     M3R_TRY(res_gemm(ws.enc16 + ws.row0[g] * w->enc_dim, w->enc_dim, w->embed_w, w->enc_dim, w->embed_b, nullptr, x0,
-                     w->image2_embed, gr.n_views * gr.N, first, Mg, ws.row0[g]));
+                     w->image2_embed, gr.n_views * gr.N, first, Mg, ws.row0[g], f8));
   }
 
   // ---- feedback + memory append (feedback_mechanism.py:39-53, decoder.py:323-330), enqueued on stream `st` once
@@ -319,12 +364,15 @@ static int decoder_forward(const m3r_decoder_weights* w, const m3r_decoder_call*
     const float* off = nullptr;
     if (w->feedback) {
       const float* last = ws.snap + (int64_t)(depth - 1) * M * D;
-      M3R_TRY(m3r_normalize16(last, D, nullptr, 0, 0, 1, w->fb_ln_eps, M, D, ws.hfb16, D, bf, st));
+      const float* fb1_s = f8 ? w8->fb1_s : nullptr;
+      M3R_TRY(normalize(f8, last, nullptr, 0, 1, w->fb_ln_eps, M, D, ws.hfb16, bf, st));
       if (w->feedback == 1) {
-        M3R_TRY(gemm(ws.hfb16, D, w->fb1_w, D, M, 4 * D, D, bf, w->fb1_b, M3R_ACT_GELU, nullptr, 0, ws.mlpfb16, 4 * D, M3R_OUT_16, st));
+        M3R_TRY(gemm(ws.hfb16, D, w->fb1_w, D, M, 4 * D, D, bf, w->fb1_b, M3R_ACT_GELU, nullptr, 0, ws.mlpfb16, 4 * D, M3R_OUT_16, st,
+                     nullptr, 0, 0, nullptr, 1, 0, 0, 0, 0, nullptr, fb1_s));
         M3R_TRY(gemm(ws.mlpfb16, 4 * D, w->fb2_w, 4 * D, M, D, 4 * D, bf, w->fb2_b, 0, nullptr, 0, ws.off, D, M3R_OUT_F32, st));
       } else {
-        M3R_TRY(gemm(ws.hfb16, D, w->fb1_w, D, M, D, D, bf, w->fb1_b, 0, nullptr, 0, ws.off, D, M3R_OUT_F32, st));
+        M3R_TRY(gemm(ws.hfb16, D, w->fb1_w, D, M, D, D, bf, w->fb1_b, 0, nullptr, 0, ws.off, D, M3R_OUT_F32, st,
+                     nullptr, 0, 0, nullptr, 1, 0, 0, 0, 0, nullptr, fb1_s));
       }
       off = ws.off;
     }
@@ -355,17 +403,20 @@ static int decoder_forward(const m3r_decoder_weights* w, const m3r_decoder_call*
     // kv: ONE normalisation over the [depth * M] rows of all levels, then the K|V projections of all levels as one
     // grouped GEMM (weights = rows [3D,5D) of each block's stacked a_w) whose epilogue writes the stored rows - and, in the
     // multi-GPU schedule, every rank's copy of them - in place
-    M3R_TRY(m3r_normalize16(ws.snap, D, off, D, (depth - 1) * M, M, w->ln_eps, depth * M, D, ws.hpost16, D, bf, st));
+    M3R_TRY(normalize(f8, ws.snap, off, (depth - 1) * M, M, w->ln_eps, depth * M, D, ws.hpost16, bf, st));
     bool stacked = depth <= M3R_MAX_GROUPS;
     for (int l = 1; l < depth && stacked; ++l)
-      stacked = w->blocks[l].a_w == reinterpret_cast<const uint16_t*>(w->blocks[0].a_w) + (int64_t)l * 5 * D * D &&
-                w->blocks[l].a_b == w->blocks[0].a_b + (int64_t)l * 5 * D;
+      stacked = w->blocks[l].a_w == reinterpret_cast<const uint8_t*>(w->blocks[0].a_w) + (int64_t)l * 5 * D * D * asz &&
+                w->blocks[l].a_b == w->blocks[0].a_b + (int64_t)l * 5 * D &&
+                (!f8 || w8->blocks[l].a_s == w8->blocks[0].a_s + (int64_t)l * 5 * D);
     for (int g = 0; g < G; ++g) {
       const m3r_dec_group& gr = c->groups[g];
       const int Mg = B * gr.n_views * gr.N;
       m3r_gemm_args a = {};
       a.lda = D; a.ldw = D; a.M = Mg; a.N = 2 * D; a.K = D; a.is_bf16 = bf; a.ldc = 2 * D; a.out_dtype = M3R_OUT_16;
       a.rows_per_batch = gr.n_views * gr.N; a.batch_stride_rows = c->mem_out_bstride_rows; a.w_static = 1; a.n_peer_out = c->n_peers;
+      m3r_gemm_e4m3_args e8 = {};
+      e8.a_e4m3 = f8;
       const int64_t orow = (int64_t)(c->new_only ? 0 : Nm) + ws.tok0[g];
       if (stacked && G == 1) {
         m3r_gemm_group grp = {};
@@ -373,21 +424,23 @@ static int decoder_forward(const m3r_decoder_weights* w, const m3r_decoder_call*
         // next to the main chain (side stream): leave the SMs a LayerNorm-emitting GEMM needs (one wave of 128x64 tiles)
         const int left = num_sms() - tiles_m * (D / 64);
         grp.max_ctas = left > 32 ? left : 32;
-        a.A = ws.hpost16; a.W = reinterpret_cast<const uint16_t*>(w->blocks[0].a_w) + (int64_t)3 * D * D; a.bias = w->blocks[0].a_b + 3 * D;
+        a.A = ws.hpost16; a.W = a_kv(w->blocks[0]); a.bias = w->blocks[0].a_b + 3 * D;
+        e8.w_scale = s_of(0, 1);                            // indexed by the stacked W row, like W: group l at l * 5D
         for (int l = 0; l < depth; ++l) {
           grp.out[l] = reinterpret_cast<uint16_t*>(c->mem_out[l]) + orow * 2 * D;
           for (int r = 0; r < c->n_peers; ++r)
             grp.peer_out[l * M3R_MAX_PEERS + r] = reinterpret_cast<uint16_t*>(c->peer_mem[r * depth + l]) + ws.tok0[g] * 2 * D;
         }
-        M3R_TRY(m3r_gemm_grouped(&a, &grp, st));
+        M3R_TRY(m3r_gemm_grouped_e4m3(&a, &grp, &e8, st));
       } else {
         for (int l = 0; l < depth; ++l) {
           const m3r_dec_block& b = w->blocks[l];
-          a.A = ws.hpost16 + ((int64_t)l * M + ws.row0[g]) * D;
-          a.W = reinterpret_cast<const uint16_t*>(b.a_w) + (int64_t)3 * D * D; a.bias = b.a_b + 3 * D;
+          a.A = reinterpret_cast<const uint8_t*>(ws.hpost16) + ((int64_t)l * M + ws.row0[g]) * D * (f8 ? 1 : 2);
+          a.W = a_kv(b); a.bias = b.a_b + 3 * D;
+          e8.w_scale = s_of(l, 1);
           a.out = reinterpret_cast<uint16_t*>(c->mem_out[l]) + orow * 2 * D;
           for (int r = 0; r < c->n_peers; ++r) a.peer_out[r] = reinterpret_cast<uint16_t*>(c->peer_mem[r * depth + l]) + ws.tok0[g] * 2 * D;
-          M3R_TRY(m3r_gemm(&a, st));
+          M3R_TRY(m3r_gemm_e4m3(&a, &e8, st));
         }
       }
     }
@@ -411,14 +464,15 @@ static int decoder_forward(const m3r_decoder_weights* w, const m3r_decoder_call*
     const int ldb = ws.merged ? 5 * D : 3 * D;
     // ---- h16 = n(X_l): first GEMM = self-attention q|k|v (RoPE on q,k) [+ pre-feedback K|V of the new tokens, the second
     // key segment of the cross-attention (decoder.py:306, layers.py:81-88)]
-    M3R_TRY(gemm(ws.h16, D, b.a_w, D, M, ldb, D, bf, b.a_b, 0, nullptr, 0, ws.big16, ldb, M3R_OUT_16, stream, ws.rope, 2 * D, M));
+    M3R_TRY(gemm(ws.h16, D, b.a_w, D, M, ldb, D, bf, b.a_b, 0, nullptr, 0, ws.big16, ldb, M3R_OUT_16, stream, ws.rope, 2 * D, M,
+                 nullptr, 1, 0, 0, 0, 0, nullptr, s_of(l, 0)));
     if (!c->render && !ws.merged) {
       for (int g = 0; g < G; ++g) {
         const m3r_dec_group& gr = c->groups[g];
         const int Mg = B * gr.n_views * gr.N;
-        M3R_TRY(gemm(ws.h16 + ws.row0[g] * D, D, reinterpret_cast<const uint16_t*>(b.a_w) + (int64_t)3 * D * D, D, Mg, 2 * D, D, bf, b.a_b + 3 * D, 0,
+        M3R_TRY(gemm(reinterpret_cast<const uint8_t*>(ws.h16) + ws.row0[g] * D * asz, D, a_kv(b), D, Mg, 2 * D, D, bf, b.a_b + 3 * D, 0,
                      nullptr, 0, ws.kvnew + ws.tok0[g] * 2 * D, 2 * D, M3R_OUT_16, stream, nullptr, 0, 0, nullptr, 1, 0,
-                     gr.n_views * gr.N, Nt));
+                     gr.n_views * gr.N, Nt, 0, nullptr, s_of(l, 1)));
       }
     }
     if (mode != M3R_MEM_KV && Nm > 0) {
@@ -446,9 +500,10 @@ static int decoder_forward(const m3r_decoder_weights* w, const m3r_decoder_call*
       M3R_TRY(m3r_attention(&at, stream));
     }
     // x_t = X_l + proj(SA), h16 = n(x_t)
-    M3R_TRY(res_gemm(ws.att16, D, b.proj_w, D, b.proj_b, xin, xt, nullptr, 1, 0, M, 0));
+    M3R_TRY(res_gemm(ws.att16, D, b.proj_w, D, b.proj_b, xin, xt, nullptr, 1, 0, M, 0, f8));
     // ---- memory cross-attention (layers.py:92-97, attention.py:139-149): q = projq(LN2(x)), K|V = memory (+ new)
-    M3R_TRY(gemm(ws.h16, D, b.q_w, D, M, D, D, bf, b.q_b, 0, nullptr, 0, ws.q16, D, M3R_OUT_16, stream));
+    M3R_TRY(gemm(ws.h16, D, b.q_w, D, M, D, D, bf, b.q_b, 0, nullptr, 0, ws.q16, D, M3R_OUT_16, stream,
+                 nullptr, 0, 0, nullptr, 1, 0, 0, 0, 0, nullptr, s_of(l, 2)));
     // context parallel: does this rank hold any key for this call?  (its memory shard, or - on rank 0 - the other views'
     // new tokens of a multi-view call)
     const bool cp_new_keys = cp && !c->render && c->cp_rank == 0 && n_total > 1;
@@ -496,11 +551,12 @@ static int decoder_forward(const m3r_decoder_weights* w, const m3r_decoder_call*
       }
       M3R_TRY(m3r_attn_merge(po, pml, c->cp_world, M, Hh, ws.att16, D, bf, stream));
     }
-    M3R_TRY(res_gemm(ws.att16, D, b.cproj_w, D, b.cproj_b, xt, xt, nullptr, 1, 0, M, 0));
+    M3R_TRY(res_gemm(ws.att16, D, b.cproj_w, D, b.cproj_b, xt, xt, nullptr, 1, 0, M, 0, f8));
     // ---- MLP (layers.py:98)
     M3R_TRY(gemm(ws.h16, D, b.fc1_w, D, M, w->mlp_hidden, D, bf, b.fc1_b, M3R_ACT_GELU, nullptr, 0, ws.mlp16, w->mlp_hidden,
-                 M3R_OUT_16, stream));
-    M3R_TRY(res_gemm(ws.mlp16, w->mlp_hidden, b.fc2_w, w->mlp_hidden, b.fc2_b, xt, xout, nullptr, 1, 0, M, 0));
+                 M3R_OUT_16, stream, nullptr, 0, 0, nullptr, 1, 0, 0, 0, 0, nullptr, s_of(l, 3)));
+    // (the last block's LayerNorm feeds the 16-bit head)
+    M3R_TRY(res_gemm(ws.mlp16, w->mlp_hidden, b.fc2_w, w->mlp_hidden, b.fc2_b, xt, xout, nullptr, 1, 0, M, 0, f8 && l + 1 < depth));
     M3R_TRY(maybe_append(l + 1));
   }
 
@@ -540,16 +596,32 @@ __global__ void mem_commit_kernel(const __grid_constant__ CommitArgs a, const in
 
 extern "C" int m3r_decoder_forward(const m3r_decoder_weights* w, const m3r_decoder_call* c, void* workspace,
                                    int64_t workspace_bytes, void* stream) {
-  return decoder_forward(w, c, nullptr, workspace, workspace_bytes, stream);
+  return decoder_forward(w, nullptr, c, nullptr, workspace, workspace_bytes, stream);
 }
 
-extern "C" int m3r_decoder_forward_ragged(const m3r_decoder_weights* w, const m3r_decoder_call* c, const int32_t* nm_scene,
-                                          void* workspace, int64_t workspace_bytes, void* stream) {
+static int check_ragged(const m3r_decoder_call* c, const int32_t* nm_scene) {
   if (!c || !nm_scene) return set_error("decoder_forward_ragged: null pointer");
   if (c->mem_mode != M3R_MEM_KV || !c->new_only || c->render || c->n_peers != 0 || c->cp_world > 1)
     return set_error("decoder_forward_ragged: only memory_mode kv with new_only (no render, peers or context parallel)");
   if (c->Nm < 1 || c->is_init) return set_error("decoder_forward_ragged: needs a memory (Nm = the longest, >= 1)");
-  return decoder_forward(w, c, nm_scene, workspace, workspace_bytes, stream);
+  return 0;
+}
+
+extern "C" int m3r_decoder_forward_ragged(const m3r_decoder_weights* w, const m3r_decoder_call* c, const int32_t* nm_scene,
+                                          void* workspace, int64_t workspace_bytes, void* stream) {
+  if (check_ragged(c, nm_scene)) return 1;
+  return decoder_forward(w, nullptr, c, nm_scene, workspace, workspace_bytes, stream);
+}
+
+extern "C" int m3r_decoder_forward_e4m3(const m3r_decoder_weights* w, const m3r_decoder_e4m3* w8, const m3r_decoder_call* c,
+                                        const int32_t* nm_scene, void* workspace, int64_t workspace_bytes, void* stream) {
+  if (!w || !w8 || !w8->blocks) return set_error("decoder_forward_e4m3: null pointer");
+  if (!w->is_bf16) return set_error("decoder_forward_e4m3: the 16-bit operands of the e4m3 decoder are bf16 (is_bf16 = 1)");
+  for (int l = 0; l < w->depth; ++l)
+    if (!w8->blocks[l].a_s || !w8->blocks[l].q_s || !w8->blocks[l].fc1_s) return set_error("decoder_forward_e4m3: block %d has no weight scales", l);
+  if (w->feedback && !w8->fb1_s) return set_error("decoder_forward_e4m3: feedback weights have no scales");
+  if (nm_scene && check_ragged(c, nm_scene)) return 1;
+  return decoder_forward(w, w8, c, nm_scene, workspace, workspace_bytes, stream);
 }
 
 extern "C" int m3r_mem_commit(void* const* arena, const void* const* staged, int32_t depth, int32_t B, int32_t Nt, int32_t width,

@@ -108,10 +108,12 @@ int make_tmap_2d(CUtensorMap* out, const void* base, int is_bf16, uint64_t cols,
   if (!enc) return set_error("cuTensorMapEncodeTiled is unavailable (no CUDA driver?)");
   if ((reinterpret_cast<uintptr_t>(base) & 15) != 0) return set_error("TMA base pointer must be 16-byte aligned");
   cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {ld * (fp32 ? 4 : 2)};
+  const bool e4m3 = !fp32 && is_bf16 == TMAP_E4M3;
+  cuuint64_t strides[1] = {ld * (fp32 ? 4 : e4m3 ? 1 : 2)};
   cuuint32_t box[2] = {box_cols, box_rows};
   cuuint32_t estr[2] = {1, 1};
   const CUtensorMapDataType dt = fp32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                      : e4m3 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
                                       : (is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
   CUresult r = enc(out, dt, 2,
                    const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,

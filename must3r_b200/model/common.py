@@ -43,6 +43,18 @@ class DecoderWeights(C.Structure):
                 ("head_w", C.c_void_p), ("head_b", C.c_void_p)]
 
 
+class EncBlockE4M3(C.Structure):
+    _fields_ = [("qkv_s", C.c_void_p), ("fc1_s", C.c_void_p)]
+
+
+class DecBlockE4M3(C.Structure):
+    _fields_ = [("a_s", C.c_void_p), ("q_s", C.c_void_p), ("fc1_s", C.c_void_p)]
+
+
+class DecoderE4M3(C.Structure):
+    _fields_ = [("blocks", C.POINTER(DecBlockE4M3)), ("fb1_s", C.c_void_p)]
+
+
 class DecGroup(C.Structure):
     _fields_ = [("n_views", C.c_int32), ("N", C.c_int32), ("H", C.c_int32), ("W", C.c_int32),
                 ("x_enc", C.c_void_p), ("pos", C.c_void_p), ("pointmaps", C.c_void_p)]
@@ -71,6 +83,10 @@ _lib.SIGNATURES.update({
     "m3r_decoder_forward": (C.c_int, [C.POINTER(DecoderWeights), C.POINTER(DecoderCall), C.c_void_p, C.c_int64, C.c_void_p]),
     "m3r_decoder_forward_ragged": (C.c_int, [C.POINTER(DecoderWeights), C.POINTER(DecoderCall), C.c_void_p, C.c_void_p,
                                              C.c_int64, C.c_void_p]),
+    "m3r_encoder_forward_e4m3": (C.c_int, [C.POINTER(EncoderWeights), C.POINTER(EncBlockE4M3), C.c_void_p, C.c_int32, C.c_int32,
+                                           C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "m3r_decoder_forward_e4m3": (C.c_int, [C.POINTER(DecoderWeights), C.POINTER(DecoderE4M3), C.POINTER(DecoderCall), C.c_void_p,
+                                           C.c_void_p, C.c_int64, C.c_void_p]),
 })
 
 _lib.apply_signatures()
@@ -80,20 +96,36 @@ _PRECISION = {"dtype": torch.float16}
 
 
 def set_precision(dtype) -> None:
-    """16-bit storage format of GEMM / attention operands and of the K|V memory.
+    """Storage format of GEMM / attention operands and of the K|V memory.
 
     ``torch.float16`` (default): 10-bit mantissa, i.e. the precision class of the TF32 matmuls the
     reference's demos enable (demo.py:12) - the parity mode.  ``torch.bfloat16``: the amp dtype of the
     reference's decoder (`--amp bf16`).  Both run at the same tensor-core rate; accumulation, LayerNorm, softmax
-    and the residual stream are fp32 either way."""
+    and the residual stream are fp32 either way.
+
+    ``torch.float8_e4m3fn`` (or ``"fp8"``): a speed mode.  The linear layers fed by a LayerNorm (encoder qkv and fc1;
+    decoder qkv, cross-attention projq, the memory projk|projv, fc1 and the feedback fc1) multiply e4m3 operands on the
+    FP8 tensor cores: the normalised rows need no scale (|y| <= sqrt(D - 1)) and each weight row has one fp32 scale.
+    Everything else - the other linear layers, attention, the K|V memory (``MUSt3R.memory_dtype()``) - runs as in
+    ``bfloat16``.  Measured speed and error: README.md, "FP8 mode"."""
     if isinstance(dtype, str):
-        dtype = {"fp16": torch.float16, "float16": torch.float16, "bf16": torch.bfloat16, "bfloat16": torch.bfloat16}[dtype]
-    assert dtype in (torch.float16, torch.bfloat16)
+        dtype = {"fp16": torch.float16, "float16": torch.float16, "bf16": torch.bfloat16, "bfloat16": torch.bfloat16,
+                 "fp8": torch.float8_e4m3fn, "float8_e4m3fn": torch.float8_e4m3fn}[dtype]
+    assert dtype in (torch.float16, torch.bfloat16, torch.float8_e4m3fn)
     _PRECISION["dtype"] = dtype
 
 
 def get_precision() -> torch.dtype:
     return _PRECISION["dtype"]
+
+
+def is_fp8(dtype) -> bool:
+    return dtype == torch.float8_e4m3fn
+
+
+def operand16(dtype) -> torch.dtype:
+    """The 16-bit format of the operands, outputs and memory of precision `dtype` (bf16 in the fp8 mode)."""
+    return torch.bfloat16 if is_fp8(dtype) else dtype
 
 
 class ActivationType(Enum):
@@ -174,12 +206,31 @@ class WeightPack:
             b = b + lin_b.detach().float()
         return w * gamma.detach().float()[None, :], b
 
+    def mat8(self, w: torch.Tensor):
+        """e4m3 copy of a [N, K] weight with one fp32 scale per row (output channel): scale = amax / 448 (1 for an
+        all-zero row), W8 = round_e4m3(W / scale) with torch.float8_e4m3fn's round-to-nearest-even.  -> (W8 ptr, scale ptr)"""
+        q, s = quantize_e4m3_rows(w)
+        self.keep += [q, s]
+        return q.data_ptr(), s.data_ptr()
+
     def vec(self, t: Optional[torch.Tensor]) -> Optional[int]:
         if t is None:
             return None
         x = t.detach().float().contiguous().reshape(-1)
         self.keep.append(x)
         return x.data_ptr()
+
+
+E4M3_MAX = 448.0
+
+
+def quantize_e4m3_rows(w: torch.Tensor):
+    """(W8 [N, K] float8_e4m3fn, scale [N] fp32) with W ~= W8 * scale[:, None] (see WeightPack.mat8)."""
+    w = w.detach().reshape(w.shape[0], -1).float()
+    amax = w.abs().amax(dim=1)
+    scale = torch.where(amax > 0, amax / E4M3_MAX, torch.ones_like(amax))
+    q = (w / scale[:, None]).clamp(-E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn).contiguous()
+    return q, scale.contiguous()
 
 
 _WS = {}

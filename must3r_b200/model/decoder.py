@@ -133,8 +133,8 @@ class MUSt3R(nn.Module):
         self._reserve_tokens, self._growth = int(n_tokens), float(growth)
 
     def memory_dtype(self):
-        """dtype of the K|V memory tensors this decoder produces (the current 16-bit operand format)."""
-        return cm.get_precision()
+        """dtype of the K|V memory tensors this decoder produces (the current 16-bit operand format; bf16 in fp8 mode)."""
+        return cm.operand16(cm.get_precision())
 
     # ---- housekeeping identical to the reference -----------------------------------------------------
     def change_memory_mode(self, memory_mode="norm_y"):
@@ -167,10 +167,16 @@ class MUSt3R(nn.Module):
         if self._pack is None or self._pack[0] != key:
             p = cm.WeightPack()
             D = self.embed_dim
+            fp8, d16 = cm.is_fp8(dtype), cm.operand16(dtype)
+            dev = self.norm_dec.weight.device
             blocks = (cm.DecBlock * self.depth)()
-            a_w_all = torch.empty((self.depth, 5 * D, D), dtype=dtype, device=self.norm_dec.weight.device)
-            a_b_all = torch.empty((self.depth, 5 * D), dtype=torch.float32, device=self.norm_dec.weight.device)
-            p.keep += [a_w_all, a_b_all]
+            # fp8: the LayerNorm-fed weights (a_w, q_w, fc1_w, fb1_w) are e4m3 with one fp32 scale per row
+            w8 = cm.DecoderE4M3() if fp8 else None
+            blocks8 = (cm.DecBlockE4M3 * self.depth)() if fp8 else None
+            a_w_all = torch.empty((self.depth, 5 * D, D), dtype=dtype, device=dev)
+            a_b_all = torch.empty((self.depth, 5 * D), dtype=torch.float32, device=dev)
+            a_s_all = torch.empty((self.depth, 5 * D), dtype=torch.float32, device=dev)
+            p.keep += [a_w_all, a_b_all, a_s_all]
             esz = a_w_all.element_size()
             for i, b in enumerate(self.blocks_dec):
                 e = blocks[i]
@@ -179,44 +185,61 @@ class MUSt3R(nn.Module):
                 kv_w = torch.cat([ca.projk.weight, ca.projv.weight], 0)
                 kv_b = torch.cat([ca.projk.bias, ca.projv.bias], 0)
                 wk, bk = p.folded(kv_w, kv_b, b.norm_y.weight, b.norm_y.bias)
-                a_w_all[i, :3 * D] = wq.to(dtype)
-                a_w_all[i, 3 * D:] = wk.to(dtype)
+                if fp8:
+                    a_w_all[i, :3 * D], a_s_all[i, :3 * D] = cm.quantize_e4m3_rows(wq)
+                    a_w_all[i, 3 * D:], a_s_all[i, 3 * D:] = cm.quantize_e4m3_rows(wk)
+                    blocks8[i].a_s = a_s_all.data_ptr() + i * 5 * D * 4
+                else:
+                    a_w_all[i, :3 * D] = wq.to(dtype)
+                    a_w_all[i, 3 * D:] = wk.to(dtype)
                 a_b_all[i, :3 * D] = bq
                 a_b_all[i, 3 * D:] = bk
                 e.a_w = a_w_all.data_ptr() + i * 5 * D * D * esz
                 e.a_b = a_b_all.data_ptr() + i * 5 * D * 4
-                e.proj_w, e.proj_b = p.mat(b.attn.proj.weight, dtype), p.vec(b.attn.proj.bias)
+                e.proj_w, e.proj_b = p.mat(b.attn.proj.weight, d16), p.vec(b.attn.proj.bias)
                 wq2, bq2 = p.folded(ca.projq.weight, ca.projq.bias, b.norm2.weight, b.norm2.bias)
-                e.q_w, e.q_b = p.mat(wq2, dtype), p.vec(bq2)
-                e.cproj_w, e.cproj_b = p.mat(ca.proj.weight, dtype), p.vec(ca.proj.bias)
                 w1, b1 = p.folded(b.mlp.fc1.weight, b.mlp.fc1.bias, b.norm3.weight, b.norm3.bias)
-                e.fc1_w, e.fc1_b = p.mat(w1, dtype), p.vec(b1)
-                e.fc2_w, e.fc2_b = p.mat(b.mlp.fc2.weight, dtype), p.vec(b.mlp.fc2.bias)
+                if fp8:
+                    (e.q_w, blocks8[i].q_s), (e.fc1_w, blocks8[i].fc1_s) = p.mat8(wq2), p.mat8(w1)
+                else:
+                    e.q_w, e.fc1_w = p.mat(wq2, dtype), p.mat(w1, dtype)
+                e.q_b, e.fc1_b = p.vec(bq2), p.vec(b1)
+                e.cproj_w, e.cproj_b = p.mat(ca.proj.weight, d16), p.vec(ca.proj.bias)
+                e.fc2_w, e.fc2_b = p.mat(b.mlp.fc2.weight, d16), p.vec(b.mlp.fc2.bias)
                 e.normy_w, e.normy_b = p.vec(b.norm_y.weight), p.vec(b.norm_y.bias)
-                e.kv_w, e.kv_b = p.mat(kv_w, dtype), p.vec(kv_b)          # memory_mode norm_y / raw: projected at use
+                e.kv_w, e.kv_b = p.mat(kv_w, d16), p.vec(kv_b)          # memory_mode norm_y / raw: projected at use
             w = cm.DecoderWeights()
             w.enc_dim, w.embed_dim, w.depth, w.num_heads = self.enc_embed_dim, self.embed_dim, self.depth, self.attn_num_heads
             w.mlp_hidden, w.out_dim = self.mlp_hidden, self.output_dim
             w.ln_eps, w.rope_base, w.rope_f0 = self.ln_eps, self.rope_base, self.rope_f0
-            w.is_bf16 = 1 if dtype == torch.bfloat16 else 0
-            w.embed_w, w.embed_b = p.mat(self.feat_embed_enc_to_dec.weight, dtype), p.vec(self.feat_embed_enc_to_dec.bias)
+            w.is_bf16 = 1 if d16 == torch.bfloat16 else 0
+            w.embed_w, w.embed_b = p.mat(self.feat_embed_enc_to_dec.weight, d16), p.vec(self.feat_embed_enc_to_dec.bias)
             w.image2_embed = p.vec(self.image2_embed)
             w.blocks = blocks
             if self.feedback_type == 'single_mlp':
                 w.feedback, w.fb_ln_eps = 1, self.feedback_norm.eps
                 f1, fb = p.folded(self.feedback_layer.fc1.weight, self.feedback_layer.fc1.bias, self.feedback_norm.weight, self.feedback_norm.bias)
-                w.fb1_w, w.fb1_b = p.mat(f1, dtype), p.vec(fb)
-                w.fb2_w, w.fb2_b = p.mat(self.feedback_layer.fc2.weight, dtype), p.vec(self.feedback_layer.fc2.bias)
+                w.fb1_w, w.fb1_b = self._fb1(p, f1, dtype, w8), p.vec(fb)
+                w.fb2_w, w.fb2_b = p.mat(self.feedback_layer.fc2.weight, d16), p.vec(self.feedback_layer.fc2.bias)
             elif self.feedback_type == 'single_linear':
                 w.feedback, w.fb_ln_eps = 2, self.feedback_norm.eps
                 f1, fb = p.folded(self.feedback_layer.weight, self.feedback_layer.bias, self.feedback_norm.weight, self.feedback_norm.bias)
-                w.fb1_w, w.fb1_b = p.mat(f1, dtype), p.vec(fb)
+                w.fb1_w, w.fb1_b = self._fb1(p, f1, dtype, w8), p.vec(fb)
             else:
                 w.feedback, w.fb_ln_eps = 0, 1e-5
             hw, hb = p.folded(self.head_dec.proj.weight, self.head_dec.proj.bias, self.norm_dec.weight, self.norm_dec.bias)
-            w.head_w, w.head_b = p.mat(hw, dtype), p.vec(hb)
-            self._pack = (key, w, blocks, p)
+            w.head_w, w.head_b = p.mat(hw, d16), p.vec(hb)
+            if fp8:
+                w8.blocks = blocks8
+            self._pack = (key, w, blocks, p, w8, blocks8)
         return self._pack[1]
+
+    @staticmethod
+    def _fb1(p, f1, dtype, w8):
+        if w8 is None:
+            return p.mat(f1, dtype)
+        ptr, w8.fb1_s = p.mat8(f1)
+        return ptr
 
     # ---- forward -------------------------------------------------------------------------------------
     @torch.no_grad()
@@ -262,8 +285,9 @@ class MUSt3R(nn.Module):
         if not x[0].is_cuda:
             raise RuntimeError("must3r_b200.MUSt3R runs on CUDA only (no CPU fallback)")
         dev = x[0].device
-        dtype = cm.get_precision()
-        w = self._packed(dtype)
+        w = self._packed(cm.get_precision())
+        w8 = self._pack[4]
+        dtype = self.memory_dtype()
         lib = _lib.lib()
         D, G = self.embed_dim, len(x)
         mem_D = 2 * D if self.memory_mode == "kv" else D                  # decoder.py:189,277
@@ -375,7 +399,11 @@ class MUSt3R(nn.Module):
         nbytes = lib.m3r_decoder_workspace_bytes(C.byref(w), C.byref(call))
         with torch.cuda.device(dev):           # the library keys its per-stream state (side streams, scratch) on the current device
             ws = cm.workspace(dev, nbytes, "dec")
-            if nm_scene is None:
+            if w8 is not None:
+                _lib.check(lib.m3r_decoder_forward_e4m3(C.byref(w), C.byref(w8), C.byref(call), None if nm_scene is None else
+                                                        C.c_void_p(nm_scene.data_ptr()), C.c_void_p(ws.data_ptr()),
+                                                        ws.numel(), cm.stream_ptr(dev)), "decoder_forward_e4m3")
+            elif nm_scene is None:
                 _lib.check(lib.m3r_decoder_forward(C.byref(w), C.byref(call), C.c_void_p(ws.data_ptr()), ws.numel(),
                                                    cm.stream_ptr(dev)), "decoder_forward")
             else:

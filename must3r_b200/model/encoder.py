@@ -84,23 +84,32 @@ class Dust3rEncoder(nn.Module):
         key = (dtype, str(self.norm_enc.weight.device))
         if self._pack is None or self._pack[0] != key:
             p = cm.WeightPack()
+            fp8, d16 = cm.is_fp8(dtype), cm.operand16(dtype)
             blocks = (cm.EncBlock * self.depth)()
+            blocks8 = (cm.EncBlockE4M3 * self.depth)() if fp8 else None
             for i, b in enumerate(self.blocks_enc):
                 e = blocks[i]
-                e.norm1_w, e.norm1_b = p.vec(b.norm1.weight), p.vec(b.norm1.bias)
-                e.qkv_w, e.qkv_b = p.mat(b.attn.qkv.weight, dtype), p.vec(b.attn.qkv.bias)
-                e.proj_w, e.proj_b = p.mat(b.attn.proj.weight, dtype), p.vec(b.attn.proj.bias)
-                e.norm2_w, e.norm2_b = p.vec(b.norm2.weight), p.vec(b.norm2.bias)
-                e.fc1_w, e.fc1_b = p.mat(b.mlp.fc1.weight, dtype), p.vec(b.mlp.fc1.bias)
-                e.fc2_w, e.fc2_b = p.mat(b.mlp.fc2.weight, dtype), p.vec(b.mlp.fc2.bias)
+                if fp8:
+                    # norm1 / norm2 folded into qkv / fc1, which take e4m3 operands (m3r_encoder_forward_e4m3)
+                    wq, bq = p.folded(b.attn.qkv.weight, b.attn.qkv.bias, b.norm1.weight, b.norm1.bias)
+                    w1, b1 = p.folded(b.mlp.fc1.weight, b.mlp.fc1.bias, b.norm2.weight, b.norm2.bias)
+                    (e.qkv_w, blocks8[i].qkv_s), e.qkv_b = p.mat8(wq), p.vec(bq)
+                    (e.fc1_w, blocks8[i].fc1_s), e.fc1_b = p.mat8(w1), p.vec(b1)
+                else:
+                    e.norm1_w, e.norm1_b = p.vec(b.norm1.weight), p.vec(b.norm1.bias)
+                    e.qkv_w, e.qkv_b = p.mat(b.attn.qkv.weight, dtype), p.vec(b.attn.qkv.bias)
+                    e.norm2_w, e.norm2_b = p.vec(b.norm2.weight), p.vec(b.norm2.bias)
+                    e.fc1_w, e.fc1_b = p.mat(b.mlp.fc1.weight, dtype), p.vec(b.mlp.fc1.bias)
+                e.proj_w, e.proj_b = p.mat(b.attn.proj.weight, d16), p.vec(b.attn.proj.bias)
+                e.fc2_w, e.fc2_b = p.mat(b.mlp.fc2.weight, d16), p.vec(b.mlp.fc2.bias)
             w = cm.EncoderWeights()
             w.embed_dim, w.depth, w.num_heads, w.mlp_hidden = self.embed_dim, self.depth, self.num_heads, self.mlp_hidden
             w.ln_eps, w.rope_base, w.rope_f0 = self.ln_eps, self.rope_base, self.rope_f0
-            w.is_bf16 = 1 if dtype == torch.bfloat16 else 0
-            w.patch_w, w.patch_b = p.mat(self.patch_embed.proj.weight, dtype), p.vec(self.patch_embed.proj.bias)
+            w.is_bf16 = 1 if d16 == torch.bfloat16 else 0
+            w.patch_w, w.patch_b = p.mat(self.patch_embed.proj.weight, d16), p.vec(self.patch_embed.proj.bias)
             w.blocks = blocks
             w.norm_w, w.norm_b = p.vec(self.norm_enc.weight), p.vec(self.norm_enc.bias)
-            self._pack = (key, w, blocks, p)
+            self._pack = (key, w, blocks, p, blocks8)
         return self._pack[1]
 
     def _positions(self, h, w, device):
@@ -157,8 +166,12 @@ class Dust3rEncoder(nn.Module):
         nbytes = lib.m3r_encoder_workspace_bytes(C.byref(w), V, H, W)
         with torch.cuda.device(img.device):
             ws = cm.workspace(img.device, nbytes, "enc")
-            _lib.check(lib.m3r_encoder_forward(C.byref(w), C.c_void_p(img.data_ptr()), V, H, W, C.c_void_p(pos1.data_ptr()),
-                                               C.c_void_p(out.data_ptr()), C.c_void_p(ws.data_ptr()), ws.numel(),
-                                               cm.stream_ptr(img.device)), "encoder_forward")
+            args = (C.c_void_p(img.data_ptr()), V, H, W, C.c_void_p(pos1.data_ptr()), C.c_void_p(out.data_ptr()),
+                    C.c_void_p(ws.data_ptr()), ws.numel(), cm.stream_ptr(img.device))
+            blocks8 = self._pack[4]
+            if blocks8 is None:
+                _lib.check(lib.m3r_encoder_forward(C.byref(w), *args), "encoder_forward")
+            else:
+                _lib.check(lib.m3r_encoder_forward_e4m3(C.byref(w), blocks8, *args), "encoder_forward_e4m3")
         return out, pos1.view(1, N, 2).expand(V, -1, -1).clone()
 
