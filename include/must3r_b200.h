@@ -541,6 +541,17 @@ typedef struct {
 int m3r_decoder_forward_e4m3(const m3r_decoder_weights* w, const m3r_decoder_e4m3* w8, const m3r_decoder_call* call,
                              const int32_t* nm_scene, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* The render pass (call->render = 1, decoder.py:307) over B scenes whose memories hold different numbers of tokens
+ * (several offline reconstructions stepped together, must3r_b200/engine/scenes.py): the n_views views of scene b in every
+ * group attend to rows [0, nm_scene[b]) of that scene's memory, nm_scene an int32 device array [B] (values clamped to
+ * [0, call->Nm]); call->Nm is the longest memory and must be >= 1, and scene b's memory rows begin at
+ * b * mem_bstride_rows.  Every layer's memory cross-attention runs as m3r_attention_ragged with kv_group = n_views.
+ * Nothing is written into the memory.  w8 = NULL runs the 16-bit decoder, otherwise the FP8 decoder of
+ * m3r_decoder_forward_e4m3.  Only memory_mode kv, no peers, no context parallel and is_init = 0; anything else is an
+ * argument error.  The workspace is m3r_decoder_workspace_bytes(w, call). */
+int m3r_decoder_render_ragged(const m3r_decoder_weights* w, const m3r_decoder_e4m3* w8, const m3r_decoder_call* call,
+                              const int32_t* nm_scene, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* Keyframe commit of several SLAM sessions in one launch: for each scene b < B whose flag keep[b * keep_stride] (int32,
  * device; e.g. the keyframe field of its m3r_slam_record) is non-zero, copy rows [0, Nt) of staged[l] + b * Nt * width
  * (the [B, Nt, width] 16-bit new_only output of m3r_decoder_forward_ragged) to rows dst_row[b] .. dst_row[b] + Nt - 1 of
@@ -550,6 +561,13 @@ int m3r_decoder_forward_e4m3(const m3r_decoder_weights* w, const m3r_decoder_e4m
 #define M3R_MAX_COMMIT 64
 int m3r_mem_commit(void* const* arena, const void* const* staged, int32_t depth, int32_t B, int32_t Nt, int32_t width,
                    const int64_t* dst_row, const int32_t* keep, int64_t keep_stride, void* stream);
+/* m3r_mem_commit of part of each staged block: rows [row0, row0 + rows) of staged[l] + b * src_stride_rows * width go to
+ * rows dst_row[b] .. dst_row[b] + rows - 1 of arena[l].  m3r_mem_commit is the case row0 = 0, rows = src_stride_rows = Nt.
+ * Used where a refinement pass overwrites a step's rows in place except those of the reference view.  Same conditions,
+ * and 0 <= row0, row0 + rows <= src_stride_rows. */
+int m3r_mem_commit_rows(void* const* arena, const void* const* staged, int32_t depth, int32_t B, int32_t row0, int32_t rows,
+                        int32_t src_stride_rows, int32_t width, const int64_t* dst_row, const int32_t* keep,
+                        int64_t keep_stride, void* stream);
 
 
 #ifdef __cplusplus

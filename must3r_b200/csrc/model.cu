@@ -581,13 +581,15 @@ struct CommitArgs {
   long long dst_row[M3R_MAX_COMMIT];
 };
 
-// grid (chunks, B, depth): level blockIdx.z of scene blockIdx.y, if its flag is set; rows * width / 8 uint4 per scene
-__global__ void mem_commit_kernel(const __grid_constant__ CommitArgs a, const int* keep, long long keep_stride, int Nt, int w16) {
+// grid (chunks, B, depth): level blockIdx.z of scene blockIdx.y, if its flag is set; rows * width / 8 uint4 per scene,
+// read from scene b's staged block (src_stride rows apart; a.src already points at the first row copied)
+__global__ void mem_commit_kernel(const __grid_constant__ CommitArgs a, const int* keep, long long keep_stride, int Nt, int w16,
+                                  long long src_stride) {
   griddep_wait();
   const int b = blockIdx.y, l = blockIdx.z;
   if (keep[(long long)b * keep_stride] == 0) return;
   const long long n = (long long)Nt * w16;
-  const uint4* src = a.src[l] + (long long)b * n;
+  const uint4* src = a.src[l] + (long long)b * src_stride * w16;
   uint4* dst = a.dst[l] + a.dst_row[b] * w16;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) dst[i] = src[i];
 }
@@ -613,29 +615,46 @@ extern "C" int m3r_decoder_forward_ragged(const m3r_decoder_weights* w, const m3
   return decoder_forward(w, nullptr, c, nm_scene, workspace, workspace_bytes, stream);
 }
 
-extern "C" int m3r_decoder_forward_e4m3(const m3r_decoder_weights* w, const m3r_decoder_e4m3* w8, const m3r_decoder_call* c,
-                                        const int32_t* nm_scene, void* workspace, int64_t workspace_bytes, void* stream) {
+static int check_e4m3(const m3r_decoder_weights* w, const m3r_decoder_e4m3* w8) {
   if (!w || !w8 || !w8->blocks) return set_error("decoder_forward_e4m3: null pointer");
   if (!w->is_bf16) return set_error("decoder_forward_e4m3: the 16-bit operands of the e4m3 decoder are bf16 (is_bf16 = 1)");
   for (int l = 0; l < w->depth; ++l)
     if (!w8->blocks[l].a_s || !w8->blocks[l].q_s || !w8->blocks[l].fc1_s) return set_error("decoder_forward_e4m3: block %d has no weight scales", l);
   if (w->feedback && !w8->fb1_s) return set_error("decoder_forward_e4m3: feedback weights have no scales");
+  return 0;
+}
+
+extern "C" int m3r_decoder_forward_e4m3(const m3r_decoder_weights* w, const m3r_decoder_e4m3* w8, const m3r_decoder_call* c,
+                                        const int32_t* nm_scene, void* workspace, int64_t workspace_bytes, void* stream) {
+  if (check_e4m3(w, w8)) return 1;
   if (nm_scene && check_ragged(c, nm_scene)) return 1;
   return decoder_forward(w, w8, c, nm_scene, workspace, workspace_bytes, stream);
 }
 
-extern "C" int m3r_mem_commit(void* const* arena, const void* const* staged, int32_t depth, int32_t B, int32_t Nt, int32_t width,
-                              const int64_t* dst_row, const int32_t* keep, int64_t keep_stride, void* stream) {
+extern "C" int m3r_decoder_render_ragged(const m3r_decoder_weights* w, const m3r_decoder_e4m3* w8, const m3r_decoder_call* c,
+                                         const int32_t* nm_scene, void* workspace, int64_t workspace_bytes, void* stream) {
+  if (!c || !nm_scene) return set_error("decoder_render_ragged: null pointer");
+  if (!c->render || c->mem_mode != M3R_MEM_KV || c->n_peers != 0 || c->cp_world > 1 || c->is_init)
+    return set_error("decoder_render_ragged: only a render call (render = 1, is_init = 0) with memory_mode kv, no peers and no context parallel");
+  if (c->Nm < 1) return set_error("decoder_render_ragged: needs a memory (Nm = the longest, >= 1)");
+  if (w8 && check_e4m3(w, w8)) return 1;
+  return decoder_forward(w, w8, c, nm_scene, workspace, workspace_bytes, stream);
+}
+
+static int mem_commit(void* const* arena, const void* const* staged, int32_t depth, int32_t B, int32_t row0, int32_t Nt,
+                      int32_t src_stride, int32_t width, const int64_t* dst_row, const int32_t* keep, int64_t keep_stride,
+                      void* stream) {
   if (!arena || !staged || !dst_row || !keep) return set_error("mem_commit: null pointer");
   if (B < 0 || B > M3R_MAX_COMMIT || depth < 1 || depth > M3R_MAX_GROUPS || Nt < 0 || width < 8 || width % 8)
     return set_error("mem_commit: B in [0, %d], depth in [1, %d], Nt >= 0 and width a positive multiple of 8", M3R_MAX_COMMIT, M3R_MAX_GROUPS);
+  if (row0 < 0 || (int64_t)row0 + Nt > src_stride) return set_error("mem_commit: rows [%d, %d) outside a staged block of %d rows", row0, row0 + Nt, src_stride);
   if (reinterpret_cast<uintptr_t>(keep) % 4) return set_error("mem_commit: keep must be 4-byte aligned");
   CommitArgs a = {};
   for (int l = 0; l < depth; ++l) {
     if (!arena[l] || !staged[l] || reinterpret_cast<uintptr_t>(arena[l]) % 16 || reinterpret_cast<uintptr_t>(staged[l]) % 16)
       return set_error("mem_commit: arena[%d] / staged[%d] null or not 16-byte aligned", l, l);
     a.dst[l] = reinterpret_cast<uint4*>(arena[l]);
-    a.src[l] = reinterpret_cast<const uint4*>(staged[l]);
+    a.src[l] = reinterpret_cast<const uint4*>(staged[l]) + (int64_t)row0 * (width / 8);
   }
   for (int b = 0; b < B; ++b) {
     if (dst_row[b] < 0) return set_error("mem_commit: dst_row[%d] < 0", b);
@@ -647,9 +666,20 @@ extern "C" int m3r_mem_commit(void* const* arena, const void* const* staged, int
   const int threads = 256;
   const int chunks = (int)std::min<long long>((n + threads - 1) / threads, 64);
   cudaError_t e = launch_pdl(mem_commit_kernel, dim3(chunks, B, depth), dim3(threads), 0, reinterpret_cast<cudaStream_t>(stream),
-                             a, keep, (long long)keep_stride, (int)Nt, w16);
+                             a, keep, (long long)keep_stride, (int)Nt, w16, (long long)src_stride);
   if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) return set_error("mem_commit launch: %s", cudaGetErrorString(e));
   count_launch();
   return 0;
+}
+
+extern "C" int m3r_mem_commit(void* const* arena, const void* const* staged, int32_t depth, int32_t B, int32_t Nt, int32_t width,
+                              const int64_t* dst_row, const int32_t* keep, int64_t keep_stride, void* stream) {
+  return mem_commit(arena, staged, depth, B, 0, Nt, Nt, width, dst_row, keep, keep_stride, stream);
+}
+
+extern "C" int m3r_mem_commit_rows(void* const* arena, const void* const* staged, int32_t depth, int32_t B, int32_t row0,
+                                   int32_t rows, int32_t src_stride_rows, int32_t width, const int64_t* dst_row,
+                                   const int32_t* keep, int64_t keep_stride, void* stream) {
+  return mem_commit(arena, staged, depth, B, row0, rows, src_stride_rows, width, dst_row, keep, keep_stride, stream);
 }

@@ -82,11 +82,22 @@ def _rgb(img):
 def _scene_from_device(x_out, imgs, true_shape, filenames):
     """Copy the results to the host in one batch of asynchronous copies and one wait; keep the device tensors on the scene
     for the point-cloud gather (inference.py:224-236 copies each tensor with a synchronising .cpu())."""
+    copies = _launch_scene_copies(x_out, imgs)
+    _sync_host_copies()
+    return _finish_scene(copies, true_shape, filenames)
+
+
+def _launch_scene_copies(x_out, imgs):
+    """Enqueue the host copies of one scene's results (no wait) -> what _finish_scene takes once they are waited for."""
     dev = {"pts3d": [o["pts3d"] for o in x_out], "pts3d_local": [o["pts3d_local"] for o in x_out],
            "conf": [o["conf"] for o in x_out], "c2w": [o["c2w"] for o in x_out], "img": list(imgs)}
     host = [{k: _to_out(v, "cpu") for k, v in o.items()} for o in x_out]
     cols = [_to_out(_rgb(im), "cpu") for im in imgs]
-    _sync_host_copies()
+    return dev, host, cols
+
+
+def _finish_scene(copies, true_shape, filenames):
+    dev, host, cols = copies
     focals = [float(o["focal"]) for o in host]
     cams2world = [o["c2w"] for o in host]
     scene = SceneState(host, [c.numpy() for c in cols], true_shape, focals, cams2world, filenames)

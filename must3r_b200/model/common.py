@@ -87,6 +87,8 @@ _lib.SIGNATURES.update({
                                            C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "m3r_decoder_forward_e4m3": (C.c_int, [C.POINTER(DecoderWeights), C.POINTER(DecoderE4M3), C.POINTER(DecoderCall), C.c_void_p,
                                            C.c_void_p, C.c_int64, C.c_void_p]),
+    "m3r_decoder_render_ragged": (C.c_int, [C.POINTER(DecoderWeights), C.POINTER(DecoderE4M3), C.POINTER(DecoderCall),
+                                            C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
 })
 
 _lib.apply_signatures()

@@ -263,10 +263,28 @@ class MUSt3R(nn.Module):
         ``mem_lengths`` (memory_mode 'kv'): B host integers, scene b's memory being rows [0, mem_lengths[b]) of
         ``current_mem[0][l][b]`` - e.g. a [B, cap, 2D] arena holding one SLAM session per scene.  The scenes are decoded
         in one call (csrc/model.cu m3r_decoder_forward_ragged), each attending only to its own rows, exactly as B separate
-        calls would; the lengths travel to the device without a host synchronisation."""
+        calls would; the lengths travel to the device without a host synchronisation.
+
+        x, pos and true_shape may also be lists with one entry per aspect-ratio group, as for ``forward_list``; the
+        pointmaps are then a list too."""
+        if isinstance(x, (list, tuple)):
+            _, pms, new_tokens = self.forward_list(list(x), list(pos), list(true_shape), current_mem, render=False,
+                                                   _new_only=True, _mem_lengths=mem_lengths)
+            return new_tokens, pms
         _, pms, new_tokens = self.forward_list([x], [pos], [true_shape], current_mem, render=False, _new_only=True,
                                                _mem_lengths=mem_lengths)
         return new_tokens, pms[0]
+
+    @torch.no_grad()
+    def render_tokens(self, x, pos, true_shape, current_mem, mem_lengths):
+        """Render call over B scenes whose memories hold different numbers of tokens (memory_mode 'kv'): x [B,n,N,Denc],
+        pos [B,n,N,2], true_shape [B,n,2] -> raw pointmaps [B,n,H,W,7] fp32.  ``mem_lengths``: B host integers, scene b's
+        memory being rows [0, mem_lengths[b]) of ``current_mem[0][l][b]`` (e.g. a [B, cap, 2D] arena holding one scene per
+        slot).  Each scene's views attend only to its own rows (csrc/model.cu m3r_decoder_render_ragged), as B separate
+        ``forward(..., render=True)`` calls would; nothing is written into the memory, and the lengths travel to the device
+        without a host synchronisation."""
+        _, pms = self.forward_list([x], [pos], [true_shape], current_mem, render=True, _mem_lengths=mem_lengths)
+        return pms[0]
 
     @torch.no_grad()
     def update_tokens_to_peers(self, x, pos, true_shape, current_mem, peer_ptrs):
@@ -336,8 +354,8 @@ class MUSt3R(nn.Module):
         nm_scene = None
         if _mem_lengths is not None:
             lengths = [int(n) for n in _mem_lengths]
-            if self.memory_mode != "kv" or not _new_only or current_mem is None or _peer_ptrs or _cp is not None:
-                raise ValueError("mem_lengths needs memory_mode='kv', a memory and update_tokens")
+            if self.memory_mode != "kv" or not (_new_only or render) or current_mem is None or _peer_ptrs or _cp is not None:
+                raise ValueError("mem_lengths needs memory_mode='kv', a memory and update_tokens or render_tokens")
             if len(lengths) != B or min(lengths) < 0 or max(lengths) < 1 or max(lengths) > Nm:
                 raise ValueError(f"mem_lengths {lengths}: one length in [0, {Nm}] per scene ({B}), the longest >= 1")
             Nm = max(lengths)
@@ -399,7 +417,11 @@ class MUSt3R(nn.Module):
         nbytes = lib.m3r_decoder_workspace_bytes(C.byref(w), C.byref(call))
         with torch.cuda.device(dev):           # the library keys its per-stream state (side streams, scratch) on the current device
             ws = cm.workspace(dev, nbytes, "dec")
-            if w8 is not None:
+            if render and nm_scene is not None:
+                _lib.check(lib.m3r_decoder_render_ragged(C.byref(w), None if w8 is None else C.byref(w8), C.byref(call),
+                                                         C.c_void_p(nm_scene.data_ptr()), C.c_void_p(ws.data_ptr()),
+                                                         ws.numel(), cm.stream_ptr(dev)), "decoder_render_ragged")
+            elif w8 is not None:
                 _lib.check(lib.m3r_decoder_forward_e4m3(C.byref(w), C.byref(w8), C.byref(call), None if nm_scene is None else
                                                         C.c_void_p(nm_scene.data_ptr()), C.c_void_p(ws.data_ptr()),
                                                         ws.numel(), cm.stream_ptr(dev)), "decoder_forward_e4m3")

@@ -21,9 +21,14 @@ from .model import MEMORY_MODES, load_model
 
 def get_args_parser():
     parser = argparse.ArgumentParser(prog="python -m must3r_b200.reconstruct")
+    return add_args(parser, lambda p: p.add_argument("--image_dir", required=True, type=str, help="image dir"))
+
+
+def add_args(parser, add_input):
+    """get_reconstruction.py's arguments; `add_input(parser)` adds the input argument(s) after --image_size."""
     parser.add_argument("--image_size", type=int, default=512, choices=[512, 224], help="image size")
 
-    parser.add_argument("--image_dir", required=True, type=str, help="image dir")
+    add_input(parser)
     parser.add_argument("--output", required=True, type=str, help="output dir")
 
     parser.add_argument("--weights", type=str, help="path to the model weights", default=None)
@@ -68,7 +73,10 @@ def get_args_parser():
 
 def parse_args(argv=None):
     parser = get_args_parser()
-    args = parser.parse_args(argv)
+    return check_args(parser, parser.parse_args(argv))
+
+
+def check_args(parser, args):
     if args.retrieval is not None:
         parser.error("--retrieval is not supported: retrieval keyframes need asmk and faiss, which are not vendored")
     if args.execution_mode == "retrieval":
@@ -103,14 +111,20 @@ def main(argv=None):
         keyframe_interval=args.keyframe_interval, slam_local_context_size=args.local_context_size,
         subsample=args.subsample, min_conf_keyframe=args.min_conf_keyframe,
         keyframe_overlap_thr=args.keyframe_overlap_thr, overlap_percentile=args.overlap_percentile)
+    write_scene(scene, args.output, args.file_type)
+    return 0
+
+
+def write_scene(scene, output, file_type):
+    """OUT/scene_{thr}.ply at every threshold of get_reconstruction.py and OUT/scene.pkl."""
+    from .engine import demo
     clouds = demo.get_3D_models_from_scene(scene, demo.THRESHOLDS)
     for thr, (pts, col) in zip(demo.THRESHOLDS, clouds):
-        path = os.path.join(args.output, f'scene_{thr}.{args.file_type}')
+        path = os.path.join(output, f'scene_{thr}.{file_type}')
         print('(exporting 3D scene to', path, f': {pts.shape[0]} points)')
         demo.write_ply(path, pts, col)
-    with open(os.path.join(args.output, 'scene.pkl'), 'wb') as f:
+    with open(os.path.join(output, 'scene.pkl'), 'wb') as f:
         pickle.dump(scene, f)
-    return 0
 
 
 if __name__ == '__main__':
