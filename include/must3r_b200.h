@@ -568,6 +568,21 @@ int m3r_mem_commit(void* const* arena, const void* const* staged, int32_t depth,
 int m3r_mem_commit_rows(void* const* arena, const void* const* staged, int32_t depth, int32_t B, int32_t row0, int32_t rows,
                         int32_t src_stride_rows, int32_t width, const int64_t* dst_row, const int32_t* keep,
                         int64_t keep_stride, void* stream);
+/* Order-preserving compaction, in place, of the memories of B scenes at every level in one launch (several videos
+ * reconstructed together, must3r_b200/engine/videos.py: the rows of frames that left the rolling window).  Scene b owns
+ * rows base_row[b] .. base_row[b] + cap - 1 of arena[l] (rows of `width` 16-bit elements; slot s of a [S, cap, width]
+ * arena has base row s * cap).  Its kept runs are runs[3k .. 3k + 2] = (src_row, dst_row, rows), int32 relative to its
+ * base, for k in [run_offset[b], run_offset[b + 1]): rows src_row .. src_row + rows - 1 move to dst_row .. dst_row + rows
+ * - 1.  The result is bitwise that of the runs applied one after another, each as buf[dst:dst+rows] =
+ * buf[src:src+rows].clone(), also where a run's source and destination overlap; only the runs' destination rows are
+ * written, and no scratch buffer is used.  Conditions (argument errors otherwise): 0 <= dst_row <= src_row,
+ * src_row + rows <= cap, each run's src_row and dst_row at or past the end of the previous run's; run_offset[0] = 0,
+ * non-decreasing, run_offset[B] <= M3R_MAX_COMPACT_RUNS; base rows >= 0, ascending and at least cap apart;
+ * B <= M3R_MAX_COMMIT, depth <= M3R_MAX_GROUPS, width % 8 == 0, every arena pointer 16-byte aligned.  arena, base_row,
+ * run_offset and runs are host arrays. */
+#define M3R_MAX_COMPACT_RUNS 128
+int m3r_mem_compact_rows(void* const* arena, int32_t depth, int32_t B, int32_t width, int64_t cap, const int64_t* base_row,
+                         const int32_t* run_offset, const int32_t* runs, void* stream);
 
 
 #ifdef __cplusplus

@@ -90,6 +90,8 @@ SIGNATURES = {
                                  C.POINTER(C.c_int64), C.c_void_p, C.c_int64, C.c_void_p]),
     "m3r_mem_commit_rows": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                       C.c_int32, C.c_int32, C.POINTER(C.c_int64), C.c_void_p, C.c_int64, C.c_void_p]),
+    "m3r_mem_compact_rows": (C.c_int, [C.POINTER(C.c_void_p), C.c_int32, C.c_int32, C.c_int32, C.c_int64,
+                                       C.POINTER(C.c_int64), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_void_p]),
     "m3r_attn_merge": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int32, C.c_int64, C.c_int32, C.c_void_p, C.c_int64,
                                  C.c_int32, C.c_void_p]),
     "m3r_attn_state_fill": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p]),

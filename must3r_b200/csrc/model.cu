@@ -594,6 +594,51 @@ __global__ void mem_commit_kernel(const __grid_constant__ CommitArgs a, const in
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) dst[i] = src[i];
 }
 
+struct CompactArgs {
+  uint4* buf[M3R_MAX_GROUPS];
+  long long base[M3R_MAX_COMMIT];
+  int run0[M3R_MAX_COMMIT + 1];
+  int3 runs[M3R_MAX_COMPACT_RUNS];      // (src_row, dst_row, rows) relative to the scene's base row
+};
+
+constexpr int COMPACT_COLS = 8;         // uint4 columns per CTA (128 bytes of a row)
+constexpr int COMPACT_LANES = 32;       // rows in flight per unrolled slot
+constexpr int COMPACT_UNROLL = 8;       // -> up to 256 rows moved per iteration
+
+// grid (column chunks, B, depth), COMPACT_COLS * COMPACT_LANES threads: columns [8 * blockIdx.x, + 8) of level blockIdx.z
+// of scene blockIdx.y, every run in order.  A CTA owns its columns for all rows, so the only hazard is inside the CTA:
+// each iteration moves m <= shift = src - dst destination rows, whose sources lie at or past the iteration's last
+// destination row (no read of the iteration meets one of its writes), and the barrier keeps the next iteration's writes
+// (which may land on rows this one read) behind this iteration's reads.  Every row moves once, no scratch.
+__global__ void __launch_bounds__(COMPACT_COLS * COMPACT_LANES) mem_compact_kernel(const __grid_constant__ CompactArgs a, int w16) {
+  griddep_wait();
+  const int b = blockIdx.y, l = blockIdx.z;
+  const int col = blockIdx.x * COMPACT_COLS + (threadIdx.x % COMPACT_COLS), lane = threadIdx.x / COMPACT_COLS;
+  const bool on = col < w16;
+  uint4* buf = a.buf[l] + a.base[b] * w16 + col;
+  for (int k = a.run0[b]; k < a.run0[b + 1]; ++k) {
+    const int src = a.runs[k].x, dst = a.runs[k].y, n = a.runs[k].z;
+    const int shift = src - dst;
+    if (shift == 0) continue;
+    const int step = min(shift, COMPACT_LANES * COMPACT_UNROLL);
+    for (int r0 = 0; r0 < n; r0 += step) {
+      const int m = min(step, n - r0);
+      uint4 v[COMPACT_UNROLL];
+#pragma unroll
+      for (int u = 0; u < COMPACT_UNROLL; ++u) {
+        const int r = lane + u * COMPACT_LANES;
+        if (on && r < m) v[u] = buf[(long long)(src + r0 + r) * w16];
+      }
+#pragma unroll
+      for (int u = 0; u < COMPACT_UNROLL; ++u) {
+        const int r = lane + u * COMPACT_LANES;
+        if (on && r < m) buf[(long long)(dst + r0 + r) * w16] = v[u];
+      }
+      __syncthreads();
+    }
+  }
+}
+
 }  // namespace m3r
 
 extern "C" int m3r_decoder_forward(const m3r_decoder_weights* w, const m3r_decoder_call* c, void* workspace,
@@ -682,4 +727,48 @@ extern "C" int m3r_mem_commit_rows(void* const* arena, const void* const* staged
                                    int32_t rows, int32_t src_stride_rows, int32_t width, const int64_t* dst_row,
                                    const int32_t* keep, int64_t keep_stride, void* stream) {
   return mem_commit(arena, staged, depth, B, row0, rows, src_stride_rows, width, dst_row, keep, keep_stride, stream);
+}
+
+extern "C" int m3r_mem_compact_rows(void* const* arena, int32_t depth, int32_t B, int32_t width, int64_t cap,
+                                    const int64_t* base_row, const int32_t* run_offset, const int32_t* runs, void* stream) {
+  if (!arena || !base_row || !run_offset || !runs) return set_error("mem_compact_rows: null pointer");
+  if (B < 0 || B > M3R_MAX_COMMIT || depth < 1 || depth > M3R_MAX_GROUPS || width < 8 || width % 8 || cap < 1)
+    return set_error("mem_compact_rows: B in [0, %d], depth in [1, %d], width a positive multiple of 8 and cap >= 1",
+                     M3R_MAX_COMMIT, M3R_MAX_GROUPS);
+  CompactArgs a = {};
+  for (int l = 0; l < depth; ++l) {
+    if (!arena[l] || reinterpret_cast<uintptr_t>(arena[l]) % 16)
+      return set_error("mem_compact_rows: arena[%d] null or not 16-byte aligned", l);
+    a.buf[l] = reinterpret_cast<uint4*>(arena[l]);
+  }
+  if (run_offset[0] != 0) return set_error("mem_compact_rows: run_offset[0] = %d, not 0", run_offset[0]);
+  for (int b = 0; b < B; ++b) {
+    if (run_offset[b + 1] < run_offset[b] || run_offset[b + 1] > M3R_MAX_COMPACT_RUNS)
+      return set_error("mem_compact_rows: run_offset must be non-decreasing and end at most at %d", M3R_MAX_COMPACT_RUNS);
+    if (base_row[b] < 0 || (b > 0 && base_row[b] < base_row[b - 1] + cap))
+      return set_error("mem_compact_rows: base_row[%d] = %lld: base rows must be >= 0, ascending and cap apart", b,
+                       (long long)base_row[b]);
+    a.base[b] = base_row[b];
+    a.run0[b] = run_offset[b];
+    for (int k = run_offset[b]; k < run_offset[b + 1]; ++k) {
+      const int32_t src = runs[3 * k], dst = runs[3 * k + 1], n = runs[3 * k + 2];
+      if (n < 0 || dst < 0 || dst > src || (int64_t)src + n > cap)
+        return set_error("mem_compact_rows: scene %d run %d (src %d, dst %d, rows %d) needs 0 <= dst_row <= src_row and "
+                         "src_row + rows <= cap (%lld)", b, k - run_offset[b], src, dst, n, (long long)cap);
+      if (k > run_offset[b] && (src < runs[3 * k - 3] + runs[3 * k - 1] || dst < runs[3 * k - 2] + runs[3 * k - 1]))
+        return set_error("mem_compact_rows: scene %d run %d out of order (runs ascending, each at or past the previous "
+                         "run's end)", b, k - run_offset[b]);
+      a.runs[k] = make_int3(src, dst, n);
+    }
+  }
+  a.run0[B] = run_offset[B];
+  if (B == 0 || run_offset[B] == 0) return 0;
+  const int w16 = width / 8;
+  const int chunks = (w16 + COMPACT_COLS - 1) / COMPACT_COLS;
+  cudaError_t e = launch_pdl(mem_compact_kernel, dim3(chunks, B, depth), dim3(COMPACT_COLS * COMPACT_LANES), 0,
+                             reinterpret_cast<cudaStream_t>(stream), a, w16);
+  if (e == cudaSuccess) e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error("mem_compact_rows launch: %s", cudaGetErrorString(e));
+  count_launch();
+  return 0;
 }

@@ -4,8 +4,8 @@
 
 For folder i it writes OUT/scene_{i}/scene_{thr}.ply and OUT/scene_{i}/scene.pkl, the files
 `python -m must3r_b200.reconstruct --image_dir DIR_i --output OUT/scene_{i}` writes.  The other arguments are
-reconstruct's.  Only --execution_mode linseq is batched (vidseq and vidslam choose their keyframes from each scene's own
-results: run reconstruct once per folder for them), and the decoder's memory_mode must be 'kv'.  --max_bs is per scene:
+reconstruct's.  Only --execution_mode linseq is batched here (must3r_b200.reconstruct_videos batches vidseq and vidslam),
+and the decoder's memory_mode must be 'kv'.  --max_bs is per scene:
 a decoder call over S folders holds up to S * max_bs views.
 """
 from __future__ import annotations
@@ -30,8 +30,8 @@ def parse_args(argv=None):
     parser = get_args_parser()
     args = check_args(parser, parser.parse_args(argv))
     if args.execution_mode != "linseq":
-        parser.error(f"--execution_mode {args.execution_mode} is not batched across scenes: run "
-                     "python -m must3r_b200.reconstruct once per folder for vidseq / vidslam")
+        parser.error(f"--execution_mode {args.execution_mode} is not batched here: "
+                     "python -m must3r_b200.reconstruct_videos batches vidseq / vidslam")
     if args.memory_mode not in (None, "kv"):
         parser.error(f"--memory_mode {args.memory_mode}: scenes are batched with memory_mode kv only")
     return args
