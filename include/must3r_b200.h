@@ -308,6 +308,18 @@ int m3r_slam_pose(const float* pts3d, float* pts3d_local, const float* conf, int
 int m3r_slam_keyframe(const float* dists, const float* conf, const float* pts3d_local, int32_t H, int32_t W, int32_t subsamp,
                       int32_t mode, double percentile, double thr, float min_conf_keyframe, int32_t is_first,
                       m3r_slam_record* rec, void* stream);
+/* Several cameras of one SLAM map in one step (must3r_b200/engine/slam_cameras.py): m3r_slam_pose over B views whose
+ * has_seq_focal[v], seq_focal[v] and is_first[v] (host arrays [B], B <= 64) are the view's own camera's; each record is
+ * bitwise what m3r_slam_pose writes for that view alone with those values.  One cluster per view. */
+int m3r_slam_pose_views(const float* pts3d, float* pts3d_local, const float* conf, int32_t B, int32_t H, int32_t W,
+                        float ppx, float ppy, const int32_t* has_seq_focal, const float* seq_focal, const int32_t* is_first,
+                        m3r_slam_record* rec, void* stream);
+/* m3r_slam_keyframe of F frames of one [H, W] shape in one launch, one cluster per frame: frame f reads dists + f * Q
+ * (Q = ceil(H/s) * ceil(W/s)), conf + f * H * W, pts3d_local + f * H * W * 3 and writes rec[f], bitwise what
+ * m3r_slam_keyframe writes for it alone with is_first[f] (host array [F], 1 <= F <= 64). */
+int m3r_slam_keyframe_frames(const float* dists, const float* conf, const float* pts3d_local, int32_t F, int32_t H, int32_t W,
+                             int32_t subsamp, int32_t mode, double percentile, double thr, float min_conf_keyframe,
+                             const int32_t* is_first, m3r_slam_record* rec, void* stream);
 
 /* Confidence-filtered point cloud of a reconstructed scene at T thresholds (must3r/demo/gradio.py:131-156
  * get_3D_model_from_scene with as_pointcloud, :91-92 the masking).  A device table of V views, each of its own H x W: */
@@ -568,6 +580,16 @@ int m3r_mem_commit(void* const* arena, const void* const* staged, int32_t depth,
 int m3r_mem_commit_rows(void* const* arena, const void* const* staged, int32_t depth, int32_t B, int32_t row0, int32_t rows,
                         int32_t src_stride_rows, int32_t width, const int64_t* dst_row, const int32_t* keep,
                         int64_t keep_stride, void* stream);
+/* Keyframe commit of the F frames of one step of a multi-camera SLAM run, whose frames were decoded together against one
+ * shared memory (must3r_b200/engine/slam_cameras.py): frame k < F whose flag keep[k * keep_stride] (int32, device; the
+ * keyframe field of its m3r_slam_record) is non-zero copies rows [0, Nt) of staged[l] + k * Nt * width (the [F, Nt, width]
+ * 16-bit new_only output of the decoder) to rows row0 + Nt * j .. row0 + Nt * (j + 1) - 1 of arena[l], j being the number
+ * of frames before k whose flag is set, for every level l < depth.  The result is bitwise that of m3r_mem_commit called
+ * frame after frame with the rows counted on the host; rows past row0 + Nt * (flags set) are not written.  The flags are
+ * read on the device.  arena, staged: host arrays [depth] of device pointers.  F <= M3R_MAX_COMMIT,
+ * depth <= M3R_MAX_GROUPS, width % 8 == 0, row0 >= 0, every arena / staged pointer 16-byte aligned, keep 4-byte aligned. */
+int m3r_mem_commit_ordered(void* const* arena, const void* const* staged, int32_t depth, int32_t F, int32_t Nt, int32_t width,
+                           int64_t row0, const int32_t* keep, int64_t keep_stride, void* stream);
 /* Order-preserving compaction, in place, of the memories of B scenes at every level in one launch (several videos
  * reconstructed together, must3r_b200/engine/videos.py: the rows of frames that left the rolling window).  Scene b owns
  * rows base_row[b] .. base_row[b] + cap - 1 of arena[l] (rows of `width` 16-bit elements; slot s of a [S, cap, width]

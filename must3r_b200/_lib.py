@@ -90,6 +90,8 @@ SIGNATURES = {
                                  C.POINTER(C.c_int64), C.c_void_p, C.c_int64, C.c_void_p]),
     "m3r_mem_commit_rows": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                       C.c_int32, C.c_int32, C.POINTER(C.c_int64), C.c_void_p, C.c_int64, C.c_void_p]),
+    "m3r_mem_commit_ordered": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int32, C.c_int32, C.c_int32,
+                                         C.c_int32, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]),
     "m3r_mem_compact_rows": (C.c_int, [C.POINTER(C.c_void_p), C.c_int32, C.c_int32, C.c_int32, C.c_int64,
                                        C.POINTER(C.c_int64), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_void_p]),
     "m3r_attn_merge": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int32, C.c_int64, C.c_int32, C.c_void_p, C.c_int64,
@@ -106,6 +108,12 @@ SIGNATURES = {
                                 C.c_int32, C.c_float, C.c_int32, C.c_void_p, C.c_void_p]),
     "m3r_slam_keyframe": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double,
                                     C.c_double, C.c_float, C.c_int32, C.c_void_p, C.c_void_p]),
+    "m3r_slam_pose_views": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float,
+                                      C.c_float, C.POINTER(C.c_int32), C.POINTER(C.c_float), C.POINTER(C.c_int32), C.c_void_p,
+                                      C.c_void_p]),
+    "m3r_slam_keyframe_frames": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                           C.c_int32, C.c_double, C.c_double, C.c_float, C.POINTER(C.c_int32), C.c_void_p,
+                                           C.c_void_p]),
     "m3r_scene_count": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p,
                                   C.c_void_p, C.c_void_p]),
     "m3r_scene_points": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p,

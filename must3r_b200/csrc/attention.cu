@@ -33,6 +33,10 @@
 // Their scores are masked like any padding; their V rows are zeroed in shared memory before P V, because P = 0 times a
 // stale NaN / inf V element is still NaN.  Splits are planned for the longest batch; each batch divides its own tiles
 // over them, and a CTA left without a tile contributes the empty state (m = -inf, l = 0) to the merge.
+//
+// Shared segment 0 (kv_bstride0 = 0 with several key batches): every batch reads the same K/V rows, so the batch becomes
+// the fastest grid dimension and the CTAs that read the same key tiles run together; each CTA computes exactly what it
+// computes in the usual order.
 #include <math.h>
 #include "ptx.cuh"
 #include "m3r_internal.h"
@@ -68,6 +72,7 @@ struct AttnParams {
   int kv_group;
   int skip_lo, skip_step, skip_len;
   int splits;                // key-range splits (>=1); blockIdx.z = b * splits + split
+  int batch_minor;           // shared segment 0: grid (B, H, query tiles * splits), blockIdx.z = query tile * splits + split
   const int* nk0_b;          // ragged: [B / kv_group] segment-0 lengths, clamped to [0, Nk0]; null = Nk0 for every batch
   float sl2;                 // scale * log2(e)
   void* O;                   // [B*Nq, H*64] 16-bit                     (splits == 1)
@@ -246,11 +251,11 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
   const int warp = threadIdx.x >> 5;
   const int wg = threadIdx.x >> 7;
   const int h = blockIdx.y;
-  const int b = blockIdx.z / p.splits, split = blockIdx.z % p.splits;
+  const int b = p.batch_minor ? blockIdx.x : blockIdx.z / p.splits, split = blockIdx.z % p.splits;
   const int kvb = b / p.kv_group;
   const int lo = p.skip_len > 0 ? p.skip_lo + (b % p.kv_group) * p.skip_step : 0;
   const int hi = p.skip_len > 0 ? lo + p.skip_len : 0;
-  const int q0 = blockIdx.x * NWG * AT_BM;
+  const int q0 = (p.batch_minor ? blockIdx.z / p.splits : blockIdx.x) * NWG * AT_BM;
 
   if (warp == TMA_WARP && elect_one()) {
     tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK0); tma_prefetch_desc(&tmV0);
@@ -427,7 +432,7 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
   constexpr int CH = 8;                   // float4 column chunks per thread
   const int n_qtiles = (p.Nq + AT_BM - 1) / AT_BM;
   const long long unit = ((long long)b * p.H + h) * n_qtiles + (q0 / AT_BM + wg);
-  const long long n_units = (long long)gridDim.z / p.splits * p.H * n_qtiles;
+  const long long n_units = p.rows_total / p.Nq * p.H * n_qtiles;
   // (a warpgroup whose rows are all past Nq has no unit of its own: it takes no part in the split bookkeeping)
   if (p.splits > 1 && q0 + wg * AT_BM < p.Nq) {
     float4* o4 = reinterpret_cast<float4*>(p.part_o) + ((long long)split * n_units + unit) * (16 * AT_BM) + (half * CH) * AT_BM + row;
@@ -529,7 +534,8 @@ template <bool BF16>
 static int launch_attn(const CUtensorMap& tmQ, const CUtensorMap& tmK0, const CUtensorMap& tmV0, const CUtensorMap& tmK1,
                        const CUtensorMap& tmV1, const AttnParams& p, int B, cudaStream_t s) {
   using Cfg = AttnCfg;
-  dim3 grid((p.Nq + Cfg::NWG * AT_BM - 1) / (Cfg::NWG * AT_BM), p.H, B * p.splits);
+  const int qtiles = (p.Nq + Cfg::NWG * AT_BM - 1) / (Cfg::NWG * AT_BM);
+  const dim3 grid = p.batch_minor ? dim3(B, p.H, qtiles * p.splits) : dim3(qtiles, p.H, B * p.splits);
   cudaError_t e = launch_pdl(attn_kernel<BF16>, grid, dim3(Cfg::THREADS), Cfg::SMEM, s, tmQ, tmK0, tmV0, tmK1, tmV1, p);
   if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) return set_error("attention launch: %s", cudaGetErrorString(e));
@@ -597,6 +603,11 @@ static int attention(const m3r_attn_args* a, const int32_t* nk0_b, void* stream)
   p.Nq = a->Nq; p.Nk0 = a->Nk0; p.Nk1 = a->Nk1; p.kv_group = a->kv_group;
   p.skip_lo = a->skip_lo; p.skip_step = a->skip_step; p.skip_len = a->skip_len;
   p.splits = splits; p.sl2 = a->scale * 1.4426950408889634f; p.nk0_b = nk0_b;
+  // one segment-0 K/V for every key batch (kv_bstride0 = 0, e.g. the frames of several cameras against one SLAM memory):
+  // the batches of one (head, query tile, key split) are launched next to each other, so that the K/V tiles they all read
+  // can be fetched from HBM once and served from L2 to the others (the effect on speed has not been measured)
+  p.batch_minor = a->Nk0 > 0 && a->kv_bstride0 == 0 && Bkv > 1 &&
+                  (long long)((a->Nq + AttnCfg::NWG * AT_BM - 1) / (AttnCfg::NWG * AT_BM)) * splits <= 65535 ? 1 : 0;
   p.O = a->O; p.ldo = a->ldo; p.H = a->H; p.rows_total = (long long)a->B * a->Nq;
   p.part_o = nullptr; p.part_ml = nullptr; p.split_cnt = nullptr;
   p.exp_o = a->export_o; p.exp_ml = reinterpret_cast<float2*>(a->export_ml);

@@ -594,6 +594,22 @@ __global__ void mem_commit_kernel(const __grid_constant__ CommitArgs a, const in
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) dst[i] = src[i];
 }
 
+// grid (chunks, F, depth): frame blockIdx.y of a step whose frames share one memory, if its flag is set, goes behind the
+// kept frames before it: row row0 + Nt * (flags set among frames < blockIdx.y).  The flags are read here, after the
+// dependency wait, so the records written by the preceding keyframe kernels need no trip through the host.
+__global__ void mem_commit_ordered_kernel(const __grid_constant__ CommitArgs a, const int* keep, long long keep_stride,
+                                          int Nt, int w16, long long row0) {
+  griddep_wait();
+  const int k = blockIdx.y, l = blockIdx.z;
+  if (keep[(long long)k * keep_stride] == 0) return;
+  int before = 0;
+  for (int j = 0; j < k; ++j) before += keep[(long long)j * keep_stride] != 0;
+  const long long n = (long long)Nt * w16;
+  const uint4* src = a.src[l] + (long long)k * n;
+  uint4* dst = a.dst[l] + (row0 + (long long)before * Nt) * w16;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) dst[i] = src[i];
+}
+
 struct CompactArgs {
   uint4* buf[M3R_MAX_GROUPS];
   long long base[M3R_MAX_COMMIT];
@@ -727,6 +743,34 @@ extern "C" int m3r_mem_commit_rows(void* const* arena, const void* const* staged
                                    int32_t rows, int32_t src_stride_rows, int32_t width, const int64_t* dst_row,
                                    const int32_t* keep, int64_t keep_stride, void* stream) {
   return mem_commit(arena, staged, depth, B, row0, rows, src_stride_rows, width, dst_row, keep, keep_stride, stream);
+}
+
+extern "C" int m3r_mem_commit_ordered(void* const* arena, const void* const* staged, int32_t depth, int32_t F, int32_t Nt,
+                                      int32_t width, int64_t row0, const int32_t* keep, int64_t keep_stride, void* stream) {
+  using namespace m3r;
+  if (!arena || !staged || !keep) return set_error("mem_commit_ordered: null pointer");
+  if (F < 0 || F > M3R_MAX_COMMIT || depth < 1 || depth > M3R_MAX_GROUPS || Nt < 0 || width < 8 || width % 8 || row0 < 0)
+    return set_error("mem_commit_ordered: F in [0, %d], depth in [1, %d], Nt >= 0, row0 >= 0 and width a positive multiple of 8",
+                     M3R_MAX_COMMIT, M3R_MAX_GROUPS);
+  if (reinterpret_cast<uintptr_t>(keep) % 4) return set_error("mem_commit_ordered: keep must be 4-byte aligned");
+  CommitArgs a = {};
+  for (int l = 0; l < depth; ++l) {
+    if (!arena[l] || !staged[l] || reinterpret_cast<uintptr_t>(arena[l]) % 16 || reinterpret_cast<uintptr_t>(staged[l]) % 16)
+      return set_error("mem_commit_ordered: arena[%d] / staged[%d] null or not 16-byte aligned", l, l);
+    a.dst[l] = reinterpret_cast<uint4*>(arena[l]);
+    a.src[l] = reinterpret_cast<const uint4*>(staged[l]);
+  }
+  if (F == 0 || Nt == 0) return 0;
+  const int w16 = width / 8;
+  const long long n = (long long)Nt * w16;
+  const int threads = 256;
+  const int chunks = (int)std::min<long long>((n + threads - 1) / threads, 64);
+  cudaError_t e = launch_pdl(mem_commit_ordered_kernel, dim3(chunks, F, depth), dim3(threads), 0,
+                             reinterpret_cast<cudaStream_t>(stream), a, keep, (long long)keep_stride, (int)Nt, w16, (long long)row0);
+  if (e == cudaSuccess) e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error("mem_commit_ordered launch: %s", cudaGetErrorString(e));
+  count_launch();
+  return 0;
 }
 
 extern "C" int m3r_mem_compact_rows(void* const* arena, int32_t depth, int32_t B, int32_t width, int64_t cap,

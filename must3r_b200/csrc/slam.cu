@@ -180,13 +180,26 @@ __device__ __forceinline__ void ray_pixel(const float* __restrict__ loc, long lo
   py = (float)(i / W) - ppy;
 }
 
+// Per-view focal state of a batch of views from several cameras (m3r_slam_pose_views); m3r_slam_pose passes one value
+// for all views and PER_VIEW = false.
+struct ViewFlags {
+  int has_seq_focal[M3R_MAX_COMMIT];
+  float seq_focal[M3R_MAX_COMMIT];
+  int is_first[M3R_MAX_COMMIT];
+};
+
+template <bool PER_VIEW>
 __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kThreads)
 slam_pose_kernel(const float* __restrict__ pts3d, float* __restrict__ pts3d_local, const float* __restrict__ conf, int H,
-                 int W, float ppx, float ppy, int has_seq_focal, float seq_focal, int is_first, m3r_slam_record* __restrict__ rec) {
+                 int W, float ppx, float ppy, int has_seq_focal_all, float seq_focal_all, int is_first_all,
+                 const __grid_constant__ ViewFlags vf, m3r_slam_record* __restrict__ rec) {
   __shared__ SlamShared sh;
   cg::cluster_group cluster = cg::this_cluster();
   const unsigned rank = cluster.block_rank();
   const int view = blockIdx.x / kCluster;
+  const int has_seq_focal = PER_VIEW ? vf.has_seq_focal[view] : has_seq_focal_all;
+  const float seq_focal = PER_VIEW ? vf.seq_focal[view] : seq_focal_all;
+  const int is_first = PER_VIEW ? vf.is_first[view] : is_first_all;
   const long long N = (long long)H * W;
   const long long chunk = (N + kCluster - 1) / kCluster;
   const long long lo = min(N, rank * chunk), hi = min(N, lo + chunk);
@@ -290,15 +303,26 @@ slam_pose_kernel(const float* __restrict__ pts3d, float* __restrict__ pts3d_loca
   cluster.sync();                         // no CTA leaves while another may still read its shared memory
 }
 
+// One cluster per frame: frame blockIdx.x / kCluster reads its own rows of dists [F, Q], conf [F, H, W] and pts3d_local
+// [F, H, W, 3] and writes rec[frame]; bit f of first_mask is frame f's is_first.  A single frame (F = 1) is
+// m3r_slam_keyframe.
 __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kThreads)
-slam_keyframe_kernel(const float* __restrict__ dists, const float* __restrict__ conf, const float* __restrict__ pts3d_local,
-                     int H, int W, int s, int mode, double q, double thr, float min_conf, int is_first,
-                     m3r_slam_record* __restrict__ rec) {
+slam_keyframe_kernel(const float* __restrict__ dists_all, const float* __restrict__ conf_all,
+                     const float* __restrict__ pts3d_local_all, int H, int W, int s, int mode, double q, double thr,
+                     float min_conf, unsigned long long first_mask, m3r_slam_record* __restrict__ rec_all) {
   __shared__ SlamShared sh;
   cg::cluster_group cluster = cg::this_cluster();
   const unsigned rank = cluster.block_rank();
+  const int frame = blockIdx.x / kCluster;
+  const int is_first = (int)((first_mask >> frame) & 1ull);
   const int ws = (W + s - 1) / s;
   const long long Q = (long long)((H + s - 1) / s) * ws;
+  const long long HW = (long long)H * W;
+  // (a null dists / pts3d_local is never read: the conf modes do not look at them)
+  const float* __restrict__ dists = dists_all + Q * frame;
+  const float* __restrict__ conf = conf_all + HW * frame;
+  const float* __restrict__ pts3d_local = pts3d_local_all + 3 * HW * frame;
+  m3r_slam_record* __restrict__ rec = rec_all + frame;
   const long long chunk = (Q + kCluster - 1) / kCluster;
   const long long lo = min(Q, rank * chunk), hi = min(Q, lo + chunk);
   int sbuf = 0, hbuf = 0;
@@ -360,25 +384,71 @@ static int check_launch(const char* what) {
 
 using namespace m3r;
 
+static int pose_args(const float* pts3d, const float* pts3d_local, const float* conf, int32_t B, int32_t H, int32_t W,
+                     const m3r_slam_record* rec) {
+  if (B <= 0 || H <= 0 || W <= 0) return set_error("slam_pose: bad shape B=%d H=%d W=%d", B, H, W);
+  if (!pts3d || !pts3d_local || !conf || !rec) return set_error("slam_pose: null pointer");
+  return 0;
+}
+
 extern "C" int m3r_slam_pose(const float* pts3d, float* pts3d_local, const float* conf, int32_t B, int32_t H, int32_t W,
                              float ppx, float ppy, int32_t has_seq_focal, float seq_focal, int32_t is_first,
                              m3r_slam_record* rec, void* stream) {
-  if (B <= 0 || H <= 0 || W <= 0) return set_error("slam_pose: bad shape B=%d H=%d W=%d", B, H, W);
-  if (!pts3d || !pts3d_local || !conf || !rec) return set_error("slam_pose: null pointer");
-  launch_pdl(slam_pose_kernel, dim3(B * kCluster), dim3(kThreads), 0, reinterpret_cast<cudaStream_t>(stream), pts3d,
-             pts3d_local, conf, (int)H, (int)W, ppx, ppy, (int)has_seq_focal, seq_focal, (int)is_first, rec);
+  if (pose_args(pts3d, pts3d_local, conf, B, H, W, rec)) return 1;
+  const ViewFlags none = {};
+  launch_pdl(slam_pose_kernel<false>, dim3(B * kCluster), dim3(kThreads), 0, reinterpret_cast<cudaStream_t>(stream), pts3d,
+             pts3d_local, conf, (int)H, (int)W, ppx, ppy, (int)has_seq_focal, seq_focal, (int)is_first, none, rec);
   return check_launch("slam_pose");
 }
 
-extern "C" int m3r_slam_keyframe(const float* dists, const float* conf, const float* pts3d_local, int32_t H, int32_t W,
-                                 int32_t subsamp, int32_t mode, double percentile, double thr, float min_conf_keyframe,
-                                 int32_t is_first, m3r_slam_record* rec, void* stream) {
+extern "C" int m3r_slam_pose_views(const float* pts3d, float* pts3d_local, const float* conf, int32_t B, int32_t H,
+                                   int32_t W, float ppx, float ppy, const int32_t* has_seq_focal, const float* seq_focal,
+                                   const int32_t* is_first, m3r_slam_record* rec, void* stream) {
+  if (pose_args(pts3d, pts3d_local, conf, B, H, W, rec)) return 1;
+  if (B > M3R_MAX_COMMIT) return set_error("slam_pose_views: B = %d views, at most %d", B, M3R_MAX_COMMIT);
+  if (!has_seq_focal || !seq_focal || !is_first) return set_error("slam_pose_views: null per-view array");
+  ViewFlags vf = {};
+  for (int v = 0; v < B; ++v) {
+    vf.has_seq_focal[v] = has_seq_focal[v];
+    vf.seq_focal[v] = seq_focal[v];
+    vf.is_first[v] = is_first[v];
+  }
+  launch_pdl(slam_pose_kernel<true>, dim3(B * kCluster), dim3(kThreads), 0, reinterpret_cast<cudaStream_t>(stream), pts3d,
+             pts3d_local, conf, (int)H, (int)W, ppx, ppy, 0, 0.f, 0, vf, rec);
+  return check_launch("slam_pose_views");
+}
+
+static int keyframe_args(const float* dists, const float* conf, const float* pts3d_local, int32_t H, int32_t W,
+                         int32_t subsamp, int32_t mode, double percentile, const m3r_slam_record* rec) {
   if (H <= 0 || W <= 0 || subsamp <= 0) return set_error("slam_keyframe: bad shape H=%d W=%d subsamp=%d", H, W, subsamp);
   if (mode < M3R_OVERLAP_NN || mode > M3R_OVERLAP_MEDIANCONF) return set_error("slam_keyframe: unknown overlap mode %d", mode);
   if (!(percentile >= 0.0 && percentile <= 100.0)) return set_error("slam_keyframe: percentile %g outside [0, 100]", percentile);
   if (!conf || !rec || (mode <= M3R_OVERLAP_NN_NORM && !dists) || (mode == M3R_OVERLAP_NN_NORM && !pts3d_local))
     return set_error("slam_keyframe: null pointer");
+  return 0;
+}
+
+extern "C" int m3r_slam_keyframe(const float* dists, const float* conf, const float* pts3d_local, int32_t H, int32_t W,
+                                 int32_t subsamp, int32_t mode, double percentile, double thr, float min_conf_keyframe,
+                                 int32_t is_first, m3r_slam_record* rec, void* stream) {
+  if (keyframe_args(dists, conf, pts3d_local, H, W, subsamp, mode, percentile, rec)) return 1;
   launch_pdl(slam_keyframe_kernel, dim3(kCluster), dim3(kThreads), 0, reinterpret_cast<cudaStream_t>(stream), dists, conf,
-             pts3d_local, (int)H, (int)W, (int)subsamp, (int)mode, percentile / 100.0, thr, min_conf_keyframe, (int)is_first, rec);
+             pts3d_local, (int)H, (int)W, (int)subsamp, (int)mode, percentile / 100.0, thr, min_conf_keyframe,
+             is_first ? 1ull : 0ull, rec);
   return check_launch("slam_keyframe");
+}
+
+extern "C" int m3r_slam_keyframe_frames(const float* dists, const float* conf, const float* pts3d_local, int32_t F,
+                                        int32_t H, int32_t W, int32_t subsamp, int32_t mode, double percentile, double thr,
+                                        float min_conf_keyframe, const int32_t* is_first, m3r_slam_record* rec,
+                                        void* stream) {
+  if (keyframe_args(dists, conf, pts3d_local, H, W, subsamp, mode, percentile, rec)) return 1;
+  if (F <= 0 || F > M3R_MAX_COMMIT) return set_error("slam_keyframe_frames: F = %d frames, 1..%d", F, M3R_MAX_COMMIT);
+  if (!is_first) return set_error("slam_keyframe_frames: null is_first");
+  unsigned long long mask = 0;
+  for (int f = 0; f < F; ++f) mask |= is_first[f] ? 1ull << f : 0ull;
+  launch_pdl(slam_keyframe_kernel, dim3(F * kCluster), dim3(kThreads), 0, reinterpret_cast<cudaStream_t>(stream), dists,
+             conf, pts3d_local, (int)H, (int)W, (int)subsamp, (int)mode, percentile / 100.0, thr, min_conf_keyframe, mask,
+             rec);
+  return check_launch("slam_keyframe_frames");
 }

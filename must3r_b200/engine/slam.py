@@ -386,10 +386,11 @@ class SLAM_MUSt3R():
             _release_tail(self.memory)        # the update of a frame that is not a keyframe is dropped
         return ret
 
-    def _record_frame(self, view, pred, fid, out):
+    def _record_frame(self, view, pred, fid, out, build_index=True):
         """Host bookkeeping of a frame once its record is known (out = the agent's update tuple; the caller updates the
-        memory): its timestamp, pose and confidence; on a keyframe its id, its confident points in the searcher and, with
-        keep_memory, its point map.  -> what __call__ returns for the frame."""
+        memory): its timestamp, pose and confidence; on a keyframe its id, its confident points in the searcher (and,
+        unless build_index is False, the searcher's index rebuilt now) and, with keep_memory, its point map.  -> what
+        __call__ returns for the frame."""
         selpts3d, pts3d, colors, depth, conf, focal, w2c, cam_center, iskeyframe = out
         self.all_timestamps.append(fid)
         self.all_poses.append(pred['slam_c2w'])
@@ -398,7 +399,8 @@ class SLAM_MUSt3R():
             self.keyframes.append(fid)
             if self.overlap_tree is not None:
                 self.overlap_tree.add_pts(selpts3d, cam_center=cam_center)
-                _index_ready(self.overlap_tree, self.device)
+                if build_index:
+                    _index_ready(self.overlap_tree, self.device)
             if self.keep_memory:
                 self.keyframe_pointmaps.append([pts3d.cpu(), colors.cpu(), conf.cpu()])
         return pts3d.cpu().numpy(), colors.cpu().numpy(), depth, conf, focal, w2c, view['true_shape'][0], iskeyframe

@@ -392,6 +392,51 @@ def slam_pose(pts3d: torch.Tensor, pts3d_local: torch.Tensor, conf: torch.Tensor
     return rec
 
 
+def slam_pose_views(pts3d: torch.Tensor, pts3d_local: torch.Tensor, conf: torch.Tensor, seq_focals, is_first,
+                    rec: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """slam_pose over B <= 64 views with one (seq_focal or None, is_first) per view, e.g. the frames of several cameras
+    with their own agents' focals (csrc/slam.cu m3r_slam_pose_views): each record is bitwise slam_pose's for that view
+    alone."""
+    _req_cuda(pts3d, pts3d_local, conf)
+    for t in (pts3d, pts3d_local, conf):
+        assert t.dtype == torch.float32 and t.is_contiguous()
+    B, H, W = conf.shape
+    assert pts3d.shape == (B, H, W, 3) and pts3d_local.shape == (B, H, W, 3)
+    assert len(seq_focals) == B and len(is_first) == B
+    if rec is None:
+        rec = torch.empty((B, SLAM_RECORD.itemsize), dtype=torch.uint8, device=conf.device)
+    assert rec.shape == (B, SLAM_RECORD.itemsize) and rec.is_contiguous()
+    has = (C.c_int32 * B)(*[int(f is not None) for f in seq_focals])
+    foc = (C.c_float * B)(*[0.0 if f is None else float(f) for f in seq_focals])
+    first = (C.c_int32 * B)(*[int(bool(x)) for x in is_first])
+    _lib.check(_lib.lib().m3r_slam_pose_views(_p(pts3d), _p(pts3d_local), _p(conf), B, H, W, W / 2, H / 2, has, foc, first,
+                                              _p(rec), _stream()), "slam_pose_views")
+    return rec
+
+
+def slam_keyframe_frames(dists: Optional[torch.Tensor], conf: torch.Tensor, pts3d_local: torch.Tensor, rec: torch.Tensor,
+                         *, subsamp: Optional[int], mode: str, percentile: float, thr: float, min_conf_keyframe: float,
+                         is_first) -> torch.Tensor:
+    """slam_keyframe of F <= 64 frames in one launch (csrc/slam.cu m3r_slam_keyframe_frames): conf [F,H,W], pts3d_local
+    [F,H,W,3] fp32 contiguous, dists [F, Q] (None for the conf modes), rec [F, SLAM_RECORD.itemsize], is_first F flags;
+    each record is bitwise slam_keyframe's for that frame alone."""
+    _req_cuda(dists, conf, pts3d_local, rec)
+    F, H, W = conf.shape
+    s = int(subsamp) if subsamp else 1
+    m = overlap_mode_id(mode)
+    assert conf.dtype == torch.float32 and conf.is_contiguous()
+    assert pts3d_local.dtype == torch.float32 and pts3d_local.is_contiguous() and pts3d_local.shape == (F, H, W, 3)
+    if m <= 1:
+        assert dists is not None and dists.dtype == torch.float32 and dists.is_contiguous()
+        assert dists.numel() == F * ((H + s - 1) // s) * ((W + s - 1) // s)
+    assert rec.shape == (F, SLAM_RECORD.itemsize) and rec.is_contiguous() and len(is_first) == F
+    first = (C.c_int32 * F)(*[int(bool(x)) for x in is_first])
+    _lib.check(_lib.lib().m3r_slam_keyframe_frames(_p(dists) if m <= 1 else None, _p(conf), _p(pts3d_local), F, H, W, s, m,
+                                                   float(percentile), float(thr), float(min_conf_keyframe), first, _p(rec),
+                                                   _stream()), "slam_keyframe_frames")
+    return rec
+
+
 SCENE_VIEW = np.dtype([("pts3d", "<u8"), ("c2w", "<u8"), ("conf", "<u8"), ("img", "<u8"), ("H", "<i4"), ("W", "<i4"),
                        ("first_tile", "<i8")])           # m3r_scene_view
 SCENE_TILE = 1024
