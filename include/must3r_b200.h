@@ -370,6 +370,50 @@ int m3r_resize_aa_bilinear_u8(const uint8_t* src, int64_t src_pitch, int64_t src
                               const int32_t* ybounds, const float* yweights, int32_t yk, int32_t out_h, float* tmp,
                               float* out, void* stream);
 
+/* ---- Baseline JPEG decoding (jpeg.cu), bit for bit what Pillow (libjpeg-turbo, JDCT_ISLOW, fancy upsampling) gives.
+ * Host: m3r_jpeg_parse reads the headers of a file held in memory; m3r_jpeg_prepare makes one pass over the entropy-
+ * coded data into a caller buffer (byte unstuffing, restart markers removed) with the Huffman / quantisation tables and
+ * the restart-segment table; m3r_jpeg_plan lays out a batch.  Device: m3r_jpeg_decode decodes the batch on `stream`. */
+typedef struct m3r_jpeg_info {
+  int32_t width, height, ncomp;
+  int32_t eligible;            /* 1: the GPU decoder takes the file (baseline / extended 8-bit Huffman, one scan, gray
+                                  or YCbCr with luma sampling 1x1, 2x1, 2x2 or 1x2 and chroma 1x1) */
+  int32_t orientation;         /* EXIF IFD0 0x0112, else XMP tiff:Orientation (Pillow's getexif); 1 when absent */
+  int32_t orientation_exact;   /* 0: the metadata is unusual enough that only Pillow can say what exif_transpose does */
+  int32_t restart_interval;    /* MCUs per restart segment, 0 = none */
+  int32_t hs[3], vs[3];        /* sampling factors */
+  int64_t scan_offset;         /* first byte of the entropy-coded data */
+  int64_t prep_bytes;          /* bytes m3r_jpeg_prepare writes at most */
+} m3r_jpeg_info;
+
+/* One prepared image of a batch.  Offsets are bytes from the start of the batch's prepared buffer (which is copied to
+ * the device as one piece); `out` is the image's device output [H, W, 3] uint8 (W, H swapped for orientations 5..8). */
+typedef struct m3r_jpeg_desc {
+  int64_t tables_off, segs_off, subs_off, stream_off, stream_bytes;
+  uint8_t* out;
+  int32_t width, height, ncomp, orientation;   /* orientation: the transpose applied on the store (1 = none) */
+  int32_t mcux, mcuy, bpm, restart_interval, nseg, nsub;
+  int32_t hs[3], vs[3];
+  /* m3r_jpeg_plan: prefix sums over the batch and workspace offsets */
+  int64_t sub_base, blk_base, pix_base, coef_off, plane_off[3];
+} m3r_jpeg_desc;
+
+/* Parse the headers; returns 0 (info filled, eligible or not) or 1 for a file that is not a JPEG at all. */
+int m3r_jpeg_parse(const uint8_t* data, int64_t size, m3r_jpeg_info* info);
+/* Fill `dst` (info->prep_bytes, 16-byte aligned) and `desc` (offsets + base_off).  Returns 0, or 2 when the entropy-coded
+ * data makes the file ineligible after all (a second scan, misnumbered or missing restart markers, no EOI). */
+int m3r_jpeg_prepare(const uint8_t* data, int64_t size, const m3r_jpeg_info* info, int32_t orientation, uint8_t* dst,
+                     int64_t base_off, m3r_jpeg_desc* desc);
+/* Fill the batch fields of `descs` and return the device workspace bytes m3r_jpeg_decode needs (-1 on error). */
+int64_t m3r_jpeg_plan(m3r_jpeg_desc* descs, int32_t n);
+/* Decode the batch: `host_descs` (planned) describe it, `dev_blob` is the device copy of the prepared buffer, whose
+ * descriptor array sits at byte `descs_off`.  status[n] (device int32) gets 0 or the M3R_JPEG_E* bits of each image. */
+int m3r_jpeg_decode(const m3r_jpeg_desc* host_descs, int32_t n, const uint8_t* dev_blob, int64_t descs_off, uint8_t* work,
+                    int64_t work_bytes, int32_t* status, void* stream);
+#define M3R_JPEG_EHUFF 1       /* a code missing from its table, or a coefficient past the end of a block */
+#define M3R_JPEG_ESHORT 2      /* a restart segment ends before its last MCU */
+#define M3R_JPEG_ESYNC 4       /* the parallel decoder did not agree with itself within its round budget */
+
 /* ===================================================================================================
  * Whole-model entry points: one call enqueues every kernel of a forward pass from C++ (no per-layer
  * Python/ctypes overhead).  Weight structs hold DEVICE pointers (16-bit matrices in nn.Linear layout,

@@ -58,6 +58,22 @@ class AttnArgs(C.Structure):
     ]
 
 
+class JpegInfo(C.Structure):
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("ncomp", C.c_int32), ("eligible", C.c_int32),
+                ("orientation", C.c_int32), ("orientation_exact", C.c_int32), ("restart_interval", C.c_int32),
+                ("hs", C.c_int32 * 3), ("vs", C.c_int32 * 3), ("scan_offset", C.c_int64), ("prep_bytes", C.c_int64)]
+
+
+class JpegDesc(C.Structure):
+    _fields_ = [("tables_off", C.c_int64), ("segs_off", C.c_int64), ("subs_off", C.c_int64), ("stream_off", C.c_int64),
+                ("stream_bytes", C.c_int64), ("out", C.c_void_p),
+                ("width", C.c_int32), ("height", C.c_int32), ("ncomp", C.c_int32), ("orientation", C.c_int32),
+                ("mcux", C.c_int32), ("mcuy", C.c_int32), ("bpm", C.c_int32), ("restart_interval", C.c_int32),
+                ("nseg", C.c_int32), ("nsub", C.c_int32), ("hs", C.c_int32 * 3), ("vs", C.c_int32 * 3),
+                ("sub_base", C.c_int64), ("blk_base", C.c_int64), ("pix_base", C.c_int64), ("coef_off", C.c_int64),
+                ("plane_off", C.c_int64 * 3)]
+
+
 # name -> (restype, argtypes); must list every symbol include/must3r_b200.h declares
 SIGNATURES = {
     "m3r_last_error": (C.c_char_p, []),
@@ -125,6 +141,12 @@ SIGNATURES = {
     "m3r_resize_aa_bilinear_u8": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32,
                                             C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
                                             C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "m3r_jpeg_parse": (C.c_int, [C.c_char_p, C.c_int64, C.POINTER(JpegInfo)]),
+    "m3r_jpeg_prepare": (C.c_int, [C.c_char_p, C.c_int64, C.POINTER(JpegInfo), C.c_int32, C.c_void_p, C.c_int64,
+                                   C.POINTER(JpegDesc)]),
+    "m3r_jpeg_plan": (C.c_int64, [C.POINTER(JpegDesc), C.c_int32]),
+    "m3r_jpeg_decode": (C.c_int, [C.POINTER(JpegDesc), C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
+                                  C.c_void_p]),
     "m3r_peer_alloc": (C.c_int, [C.c_int64, C.POINTER(C.c_void_p)]),
     "m3r_peer_free": (C.c_int, [C.c_void_p]),
     "m3r_ipc_export": (C.c_int, [C.c_void_p, C.c_void_p]),

@@ -7,9 +7,10 @@ reference's: with several folders the frames alternate between them, a folder th
 goes to the next one), and `grab()` moves every folder on by one frame.  Video files and camera streams (cv2) are not
 supported.
 
-Frames are decoded by PIL to RGB uint8 (EXIF orientation applied, as cv2.imread does).  The reference decodes with
-cv2.imread and converts BGR to RGB, so the arrays are the same for lossless formats such as PNG; for JPEG the two
-decoders may differ in the last bits.
+Frames are RGB uint8 with the EXIF orientation applied (as cv2.imread does), bitwise what PIL decodes: `decode` runs
+PIL on the host; the read-ahead decodes baseline JPEGs on the GPU (engine/jpeg.py) and everything else with PIL.  The
+reference decodes with cv2.imread and converts BGR to RGB, so the arrays are the same for lossless formats such as PNG;
+for JPEG the two decoders may differ in the last bits.
 """
 from __future__ import annotations
 
@@ -131,12 +132,13 @@ def image_size(path: str) -> Tuple[int, int]:
 
 
 class ReadAhead:
-    """Decodes `paths` in order on one host thread, up to `depth` frames ahead of the consumer, into pinned uint8
-    buffers.  `get()` copies the next frame to `device` with an asynchronous copy on the device's current stream and
-    returns the CUDA tensor [H,W,3]; it waits only when the reader is behind.  A buffer is decoded into again once the
-    event recorded after its copy has completed; that wait happens on the reader thread, so `get()` never synchronises
-    the device.  Memory stays bounded by depth + 2 frame buffers whatever the length of the sequence.  `wait_s` is the
-    time `get()` has spent waiting for the reader."""
+    """Decodes `paths` in order on one host thread, up to `depth` frames ahead of the consumer.  The reader reads each
+    file and parses it; a baseline JPEG has its compressed bytes staged in pinned memory and decoded on the GPU on the
+    reader's own stream (engine/jpeg.py, EXIF orientation applied), and the reader waits for its status word; any other
+    file (or a JPEG the GPU decoder hands back) is decoded by PIL and uploaded on the same stream.  `get()` makes the
+    device's current stream wait on the event recorded after the frame and returns the CUDA tensor [H,W,3]; it waits
+    on the host only when the reader is behind and never synchronises the device.  Memory stays bounded by depth + 2
+    frames whatever the length of the sequence.  `wait_s` is the time `get()` has spent waiting for the reader."""
 
     def __init__(self, paths: Sequence[str], device, depth: int = 4):
         self.device = torch.device(device)
@@ -144,7 +146,6 @@ class ReadAhead:
             self.device = torch.device('cuda', torch.cuda.current_device())
         self.paths = list(paths)
         nslots = depth + 2
-        self._bufs: List[Optional[torch.Tensor]] = [None] * nslots
         self._events = [torch.cuda.Event() for _ in range(nslots)]
         self._free: queue.Queue = queue.Queue()
         for s in range(nslots):
@@ -157,19 +158,25 @@ class ReadAhead:
         self._thread.start()
 
     def _reader(self):
+        from . import jpeg
         try:
             torch.cuda.set_device(self.device)
+            stream = torch.cuda.Stream(self.device)
             for path in self.paths:
                 slot = self._free.get()
                 if slot is None or self._stop.is_set():
                     return
-                self._events[slot].synchronize()        # the copy out of this buffer has finished
-                img = decode(path)
-                buf = self._bufs[slot]
-                if buf is None or buf.numel() < img.size:
-                    buf = self._bufs[slot] = torch.empty(img.size, dtype=torch.uint8, pin_memory=True)
-                buf[:img.size].numpy().reshape(img.shape)[...] = img
-                self._ready.put((slot, img.shape))
+                with torch.cuda.stream(stream):
+                    item = jpeg.Parsed(path, True)
+                    out = jpeg.decode_parsed([item], self.device)[0] if item.gpu else None
+                    if out is None:
+                        img = decode(path)
+                        buf = torch.empty(img.shape, dtype=torch.uint8, pin_memory=True)
+                        buf.numpy()[...] = img
+                        out = torch.empty(img.shape, dtype=torch.uint8, device=self.device)
+                        out.copy_(buf, non_blocking=True)
+                    self._events[slot].record(stream)
+                self._ready.put((slot, out))
         except BaseException as e:      # handed to the consumer, which raises it
             self._ready.put((None, e))
 
@@ -180,15 +187,14 @@ class ReadAhead:
         if self._next >= len(self.paths):
             raise IndexError("no frame left")
         t = time.perf_counter()
-        slot, shape = self._ready.get()
+        slot, out = self._ready.get()
         self.wait_s += time.perf_counter() - t
         if slot is None:
-            raise RuntimeError(f"decoding {self.paths[self._next]} failed") from shape
+            raise RuntimeError(f"decoding {self.paths[self._next]} failed") from out
         self._next += 1
-        n = int(np.prod(shape))
-        out = torch.empty(shape, dtype=torch.uint8, device=self.device)
-        out.copy_(self._bufs[slot][:n].view(shape), non_blocking=True)
-        self._events[slot].record(torch.cuda.current_stream(self.device))
+        consumer = torch.cuda.current_stream(self.device)
+        consumer.wait_event(self._events[slot])
+        out.record_stream(consumer)
         self._free.put(slot)
         return out
 

@@ -329,12 +329,18 @@ def _load_rgb(item):
 
 def load_images(folder_content, size, patch_size=16, verbose=True, device="cuda"):
     """The demo's load_images (must3r/demo/inference.py:63-76): a list of dict(img=[3,h,w] fp32 on `device`,
-    true_shape=np.int32([h, w])) in input order.  Items are image paths (decoded by PIL on the host, .convert('RGB')),
-    or RGB uint8 [H,W,3] numpy arrays / tensors.  Frames of one size are resized in one launch."""
+    true_shape=np.int32([h, w])) in input order.  Items are image paths or RGB uint8 [H,W,3] numpy arrays / tensors.
+    Paths are decoded as PIL's .convert('RGB') (no EXIF transpose, as the reference): baseline JPEGs on the GPU in
+    batches (engine/jpeg.py; waiting for each batch's status words is the one host wait), other files by PIL on the
+    host.  Frames of one size are resized in one launch."""
+    from . import jpeg
     dev = _device(device)
+    items = list(folder_content)
+    paths = [k for k, item in enumerate(items) if isinstance(item, (str, os.PathLike))]
+    decoded = dict(zip(paths, jpeg.decode_parsed_all([jpeg.Parsed(items[k], False) for k in paths], dev))) if paths else {}
     frames, names, groups = [], [], {}
-    for i, item in enumerate(folder_content):
-        f, name = _load_rgb(item)
+    for i, item in enumerate(items):
+        f, name = (decoded[i], str(item)) if i in decoded else _load_rgb(item)
         if f.ndim != 3 or f.shape[2] != 3:
             raise ValueError(f"item {i}: expected an RGB image [H,W,3], got shape {tuple(f.shape)}")
         frames.append(f)
@@ -344,8 +350,9 @@ def load_images(folder_content, size, patch_size=16, verbose=True, device="cuda"
     for (H, W), idx in groups.items():
         geo = _demo_geometry(size, H, W)
         group = [frames[i] for i in idx]
-        if all(isinstance(f, torch.Tensor) and f.is_cuda for f in group):
-            group = torch.stack(group)
+        if any(isinstance(f, torch.Tensor) and f.is_cuda for f in group):
+            group = torch.stack([f.to(dev) if isinstance(f, torch.Tensor) else torch.from_numpy(np.asarray(f)).to(dev)
+                                 for f in group])
         out, _ = _run("aa", group, (H, W), geo.out_hw, dev, src_box=geo.crop)
         for j, i in enumerate(idx):
             imgs[i] = dict(img=out[j], true_shape=np.int32([geo.out_hw[0], geo.out_hw[1]]))

@@ -522,3 +522,40 @@ def slam_keyframe(dists: Optional[torch.Tensor], conf: torch.Tensor, pts3d_local
                                             float(percentile), float(thr), float(min_conf_keyframe), int(bool(is_first)),
                                             _p(rec), _stream()), "slam_keyframe")
     return rec
+
+
+# ------------------------------------------------------------------------------------------- baseline JPEG decoding
+def jpeg_parse(data: bytes) -> "_lib.JpegInfo":
+    """Header facts of a JPEG held in memory (m3r_jpeg_parse); info.eligible says whether jpeg_decode takes it.  A file
+    that is not a JPEG comes back with eligible == 0."""
+    info = _lib.JpegInfo()
+    _lib.lib().m3r_jpeg_parse(data, len(data), C.byref(info))
+    return info
+
+
+def jpeg_prepare(data: bytes, info, orientation: int, dst_ptr: int, base_off: int) -> Optional["_lib.JpegDesc"]:
+    """Tables, restart segments and unstuffed entropy-coded data of one image written at host address dst_ptr
+    (info.prep_bytes bytes); the descriptor, or None when the data makes the file ineligible after all."""
+    desc = _lib.JpegDesc()
+    rc = _lib.lib().m3r_jpeg_prepare(data, len(data), C.byref(info), orientation, C.c_void_p(dst_ptr), base_off,
+                                     C.byref(desc))
+    if rc == 2:
+        return None
+    _lib.check(rc, "jpeg_prepare")
+    return desc
+
+
+def jpeg_plan(descs) -> int:
+    """Fill the batch fields of a ctypes array of JpegDesc; returns the workspace bytes jpeg_decode needs."""
+    n = _lib.lib().m3r_jpeg_plan(descs, len(descs))
+    if n < 0:
+        _lib.check(1, "jpeg_plan")
+    return n
+
+
+def jpeg_decode(descs, dev_blob: torch.Tensor, descs_off: int, work: torch.Tensor, status: torch.Tensor) -> None:
+    """Decode a planned batch on the current stream; status [n] int32 gets each image's M3R_JPEG_E* bits."""
+    _req_cuda(dev_blob, work, status)
+    assert status.dtype == torch.int32 and status.numel() >= len(descs)
+    _lib.check(_lib.lib().m3r_jpeg_decode(descs, len(descs), _p(dev_blob), descs_off, _p(work), work.numel(), _p(status),
+                                          _stream()), "jpeg_decode")
