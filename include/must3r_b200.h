@@ -414,6 +414,60 @@ int m3r_jpeg_decode(const m3r_jpeg_desc* host_descs, int32_t n, const uint8_t* d
 #define M3R_JPEG_ESHORT 2      /* a restart segment ends before its last MCU */
 #define M3R_JPEG_ESYNC 4       /* the parallel decoder did not agree with itself within its round budget */
 
+/* ---- PNG decoding (png.cu), bit for bit what Pillow's .convert('RGB') gives for 8-bit, non-interlaced L, RGB, P, LA
+ * and RGBA images.  Host: m3r_png_parse walks the chunks of a file held in memory (signature, CRCs of the chunks before
+ * the image data, zlib header); m3r_png_prepare copies the palette and the concatenated IDAT payloads into a caller
+ * buffer; m3r_png_plan lays out a batch.  Device: m3r_png_decode inflates and unfilters the batch on `stream`. */
+typedef struct m3r_png_info {
+  int32_t width, height;
+  int32_t bit_depth, color_type, interlace;
+  int32_t channels;            /* samples per pixel of the colour type: 1 (L, P), 2 (LA), 3 (RGB), 4 (RGBA) */
+  int32_t palette_entries;     /* PLTE entries, 0 when there is none */
+  int32_t eligible;            /* 1: the GPU decoder takes the file (the caller adds Pillow's size limit and, for the
+                                  EXIF transpose, has_exif / has_text) */
+  int32_t has_exif;            /* an eXIf chunk */
+  int32_t has_text;            /* a tEXt, zTXt or iTXt chunk (Pillow's getexif reads EXIF from these too) */
+  int64_t text_bytes;          /* payload bytes of those text chunks */
+  int64_t idat_bytes;          /* the zlib stream: the IDAT payloads concatenated */
+  int64_t prep_bytes;          /* bytes m3r_png_prepare writes */
+} m3r_png_info;
+
+/* One prepared image of a batch; offsets are bytes from the start of the batch's prepared buffer.  `out` is the image's
+ * device output [H, W, 3] uint8 (W, H swapped for orientations 5..8). */
+typedef struct m3r_png_desc {
+  int64_t plte_off;            /* 768 bytes: the palette as RGB triplets */
+  int64_t stream_off, stream_bytes;
+  uint8_t* out;
+  int32_t width, height, channels, color_type, palette_entries, orientation;
+  /* m3r_png_plan: the image's scanline workspace (filter byte + W * channels bytes per row) */
+  int64_t raw_off, raw_bytes;
+} m3r_png_desc;
+
+/* Parse the chunks; returns 0 (info filled, eligible or not) or 1 for a file that is not a PNG at all. */
+int m3r_png_parse(const uint8_t* data, int64_t size, m3r_png_info* info);
+/* Fill `dst` (info->prep_bytes, 16-byte aligned) and `desc` (offsets + base_off); 0, or set_error when the data is not
+ * the eligible PNG that was parsed. */
+int m3r_png_prepare(const uint8_t* data, int64_t size, const m3r_png_info* info, int32_t orientation, uint8_t* dst,
+                    int64_t base_off, m3r_png_desc* desc);
+/* Fill the workspace fields of `descs` and return the device workspace bytes m3r_png_decode needs (-1 on error). */
+int64_t m3r_png_plan(m3r_png_desc* descs, int32_t n);
+/* Decode the batch: `host_descs` (planned) describe it, `dev_blob` is the device copy of the prepared buffer, whose
+ * descriptor array sits at byte `descs_off`.  status[n] (device int32) gets 0 or the M3R_PNG_E* bits of each image. */
+int m3r_png_decode(const m3r_png_desc* host_descs, int32_t n, const uint8_t* dev_blob, int64_t descs_off, uint8_t* work,
+                   int64_t work_bytes, int32_t* status, void* stream);
+#define M3R_PNG_EBTYPE 1       /* a deflate block of type 3 */
+#define M3R_PNG_ESTORED 2      /* a stored block whose LEN is not the complement of NLEN */
+#define M3R_PNG_ECODES 4       /* more than 286 length or 30 distance codes, or code lengths over-subscribed or
+                                  incomplete (zlib allows an incomplete code only for a single code of length 1) */
+#define M3R_PNG_EREPEAT 8      /* a repeat code with no previous length, or one that runs past HLIT + HDIST */
+#define M3R_PNG_ENOEOB 16      /* a dynamic block without an end-of-block code */
+#define M3R_PNG_ESYMBOL 32     /* a code absent from its table, length symbol 286/287 or distance symbol 30/31 */
+#define M3R_PNG_EDIST 64       /* a distance before the start of the output */
+#define M3R_PNG_ELENGTH 128    /* the stream ends early, or its output is not H * (1 + W * channels) bytes */
+#define M3R_PNG_EFILTER 256    /* a scanline filter type above 4 */
+#define M3R_PNG_EPALETTE 512   /* a palette index past the PLTE entries */
+#define M3R_PNG_EADLER 1024    /* the Adler-32 of the output is not the stream's */
+
 /* ===================================================================================================
  * Whole-model entry points: one call enqueues every kernel of a forward pass from C++ (no per-layer
  * Python/ctypes overhead).  Weight structs hold DEVICE pointers (16-bit matrices in nn.Linear layout,

@@ -74,6 +74,19 @@ class JpegDesc(C.Structure):
                 ("plane_off", C.c_int64 * 3)]
 
 
+class PngInfo(C.Structure):
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("bit_depth", C.c_int32), ("color_type", C.c_int32),
+                ("interlace", C.c_int32), ("channels", C.c_int32), ("palette_entries", C.c_int32), ("eligible", C.c_int32),
+                ("has_exif", C.c_int32), ("has_text", C.c_int32), ("text_bytes", C.c_int64), ("idat_bytes", C.c_int64),
+                ("prep_bytes", C.c_int64)]
+
+
+class PngDesc(C.Structure):
+    _fields_ = [("plte_off", C.c_int64), ("stream_off", C.c_int64), ("stream_bytes", C.c_int64), ("out", C.c_void_p),
+                ("width", C.c_int32), ("height", C.c_int32), ("channels", C.c_int32), ("color_type", C.c_int32),
+                ("palette_entries", C.c_int32), ("orientation", C.c_int32), ("raw_off", C.c_int64), ("raw_bytes", C.c_int64)]
+
+
 # name -> (restype, argtypes); must list every symbol include/must3r_b200.h declares
 SIGNATURES = {
     "m3r_last_error": (C.c_char_p, []),
@@ -147,6 +160,12 @@ SIGNATURES = {
     "m3r_jpeg_plan": (C.c_int64, [C.POINTER(JpegDesc), C.c_int32]),
     "m3r_jpeg_decode": (C.c_int, [C.POINTER(JpegDesc), C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
                                   C.c_void_p]),
+    "m3r_png_parse": (C.c_int, [C.c_char_p, C.c_int64, C.POINTER(PngInfo)]),
+    "m3r_png_prepare": (C.c_int, [C.c_char_p, C.c_int64, C.POINTER(PngInfo), C.c_int32, C.c_void_p, C.c_int64,
+                                  C.POINTER(PngDesc)]),
+    "m3r_png_plan": (C.c_int64, [C.POINTER(PngDesc), C.c_int32]),
+    "m3r_png_decode": (C.c_int, [C.POINTER(PngDesc), C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
+                                 C.c_void_p]),
     "m3r_peer_alloc": (C.c_int, [C.c_int64, C.POINTER(C.c_void_p)]),
     "m3r_peer_free": (C.c_int, [C.c_void_p]),
     "m3r_ipc_export": (C.c_int, [C.c_void_p, C.c_void_p]),

@@ -8,7 +8,7 @@ goes to the next one), and `grab()` moves every folder on by one frame.  Video f
 supported.
 
 Frames are RGB uint8 with the EXIF orientation applied (as cv2.imread does), bitwise what PIL decodes: `decode` runs
-PIL on the host; the read-ahead decodes baseline JPEGs on the GPU (engine/jpeg.py) and everything else with PIL.  The
+PIL on the host; the read-ahead hands each file to engine/imagefiles.py, which decodes it on the GPU or with PIL.  The
 reference decodes with cv2.imread and converts BGR to RGB, so the arrays are the same for lossless formats such as PNG;
 for JPEG the two decoders may differ in the last bits.
 """
@@ -133,9 +133,9 @@ def image_size(path: str) -> Tuple[int, int]:
 
 class ReadAhead:
     """Decodes `paths` in order on one host thread, up to `depth` frames ahead of the consumer.  The reader reads each
-    file and parses it; a baseline JPEG has its compressed bytes staged in pinned memory and decoded on the GPU on the
-    reader's own stream (engine/jpeg.py, EXIF orientation applied), and the reader waits for its status word; any other
-    file (or a JPEG the GPU decoder hands back) is decoded by PIL and uploaded on the same stream.  `get()` makes the
+    file and parses it (engine/imagefiles.py, EXIF orientation applied); a file a GPU decoder takes has its compressed
+    bytes staged in pinned memory and decoded on the reader's own stream, and the reader waits for its status word;
+    any other file (or one the GPU decoder hands back) is decoded by PIL and uploaded on the same stream.  `get()` makes the
     device's current stream wait on the event recorded after the frame and returns the CUDA tensor [H,W,3]; it waits
     on the host only when the reader is behind and never synchronises the device.  Memory stays bounded by depth + 2
     frames whatever the length of the sequence.  `wait_s` is the time `get()` has spent waiting for the reader."""
@@ -158,7 +158,7 @@ class ReadAhead:
         self._thread.start()
 
     def _reader(self):
-        from . import jpeg
+        from . import imagefiles
         try:
             torch.cuda.set_device(self.device)
             stream = torch.cuda.Stream(self.device)
@@ -167,14 +167,7 @@ class ReadAhead:
                 if slot is None or self._stop.is_set():
                     return
                 with torch.cuda.stream(stream):
-                    item = jpeg.Parsed(path, True)
-                    out = jpeg.decode_parsed([item], self.device)[0] if item.gpu else None
-                    if out is None:
-                        img = decode(path)
-                        buf = torch.empty(img.shape, dtype=torch.uint8, pin_memory=True)
-                        buf.numpy()[...] = img
-                        out = torch.empty(img.shape, dtype=torch.uint8, device=self.device)
-                        out.copy_(buf, non_blocking=True)
+                    out = imagefiles.decode_frame(path, self.device)
                     self._events[slot].record(stream)
                 self._ready.put((slot, out))
         except BaseException as e:      # handed to the consumer, which raises it

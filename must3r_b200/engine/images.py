@@ -330,14 +330,16 @@ def _load_rgb(item):
 def load_images(folder_content, size, patch_size=16, verbose=True, device="cuda"):
     """The demo's load_images (must3r/demo/inference.py:63-76): a list of dict(img=[3,h,w] fp32 on `device`,
     true_shape=np.int32([h, w])) in input order.  Items are image paths or RGB uint8 [H,W,3] numpy arrays / tensors.
-    Paths are decoded as PIL's .convert('RGB') (no EXIF transpose, as the reference): baseline JPEGs on the GPU in
-    batches (engine/jpeg.py; waiting for each batch's status words is the one host wait), other files by PIL on the
-    host.  Frames of one size are resized in one launch."""
-    from . import jpeg
+    Paths are decoded as PIL's .convert('RGB') (no EXIF transpose, as the reference) by engine/imagefiles.py: the
+    files a GPU decoder takes on the GPU in batches (waiting for each batch's status words is the one host wait), other
+    files by PIL on the host.  Frames of one size are resized in one launch."""
+    from . import imagefiles
     dev = _device(device)
     items = list(folder_content)
     paths = [k for k, item in enumerate(items) if isinstance(item, (str, os.PathLike))]
-    decoded = dict(zip(paths, jpeg.decode_parsed_all([jpeg.Parsed(items[k], False) for k in paths], dev))) if paths else {}
+    with torch.cuda.device(dev):
+        decoded = dict(zip(paths, imagefiles.decode_parsed_all([imagefiles.parse(items[k], False) for k in paths],
+                                                               dev))) if paths else {}
     frames, names, groups = [], [], {}
     for i, item in enumerate(items):
         f, name = (decoded[i], str(item)) if i in decoded else _load_rgb(item)

@@ -1,6 +1,6 @@
-"""Image files decoded on the GPU: baseline JPEGs by the CUDA decoder (csrc/jpeg.cu), bitwise what
-np.asarray(PIL.Image.open(p).convert('RGB')) gives (after PIL.ImageOps.exif_transpose when asked); everything else by
-Pillow, as before.
+"""Baseline JPEGs decoded on the GPU by the CUDA decoder (csrc/jpeg.cu), bitwise what
+np.asarray(PIL.Image.open(p).convert('RGB')) gives (after PIL.ImageOps.exif_transpose when asked).  engine/imagefiles.py
+decides which decoder takes a file.
 
 The host reads each file, parses its headers and makes one pass over its entropy-coded data into a pinned buffer
 (m3r_jpeg_prepare, through ctypes, so the GIL is released); only those compressed bytes cross PCIe.  One launch sequence
@@ -13,7 +13,6 @@ from __future__ import annotations
 import ctypes as C
 from typing import List, Optional, Sequence
 
-import numpy as np
 import torch
 
 from .. import _lib, ops
@@ -27,23 +26,15 @@ def _align(n: int) -> int:
     return (n + 255) // 256 * 256
 
 
-def pillow_decode(path, exif_transpose: bool) -> np.ndarray:
-    """RGB uint8 [H,W,3] as Pillow decodes it (the reference's loaders)."""
-    import PIL.Image
-    import PIL.ImageOps
-    with PIL.Image.open(path) as im:
-        if exif_transpose:
-            im = PIL.ImageOps.exif_transpose(im)
-        return np.asarray(im.convert('RGB'))
-
-
 class Parsed:
     """One file read into memory and parsed: `info.eligible` and the orientation decide whether the GPU takes it."""
 
-    def __init__(self, path, exif_transpose: bool):
+    def __init__(self, path, exif_transpose: bool, data: Optional[bytes] = None):
         self.path, self.exif_transpose = path, exif_transpose
-        with open(path, "rb") as f:
-            self.data = f.read()
+        if data is None:
+            with open(path, "rb") as f:
+                data = f.read()
+        self.data = data
         self.info = ops.jpeg_parse(self.data)
         self.orientation = self.info.orientation if exif_transpose else 1
         self.gpu = bool(self.info.eligible) and (not exif_transpose or bool(self.info.orientation_exact))
@@ -106,7 +97,7 @@ def decode_parsed(items: Sequence[Parsed], dev: torch.device) -> List[Optional[t
         return outs
 
 
-def _batches(items: Sequence[Parsed]):
+def batches(items: Sequence[Parsed]):
     batch, work = [], 0
     for it in items:
         if batch and (len(batch) >= 64 or work + it.work_bytes > WORK_BUDGET):
@@ -118,30 +109,9 @@ def _batches(items: Sequence[Parsed]):
         yield batch
 
 
-def decode_parsed_all(items: Sequence[Parsed], dev: torch.device) -> List[torch.Tensor]:
-    """Every parsed file as a CUDA uint8 [H,W,3] tensor: the eligible ones decoded in batches on the device, the rest
-    (and any the decoder handed back) by Pillow and uploaded."""
-    out: List[Optional[torch.Tensor]] = [None] * len(items)
-    gpu = [k for k, it in enumerate(items) if it.gpu]
-    pos = 0
-    for batch in _batches([items[k] for k in gpu]):
-        for k, t in zip(gpu[pos:pos + len(batch)], decode_parsed(batch, dev)):
-            out[k] = t
-        pos += len(batch)
-    for k, it in enumerate(items):
-        if out[k] is None:
-            a = pillow_decode(it.path, it.exif_transpose)
-            out[k] = torch.from_numpy(np.array(a)).to(dev)
-    return out
-
-
 def decode_files(paths: Sequence, device="cuda", exif_transpose: bool = False) -> List[torch.Tensor]:
-    """One CUDA uint8 [H,W,3] tensor per path, bitwise equal to np.asarray(PIL.Image.open(p).convert('RGB')) (after
-    PIL.ImageOps.exif_transpose when `exif_transpose`).  Eligible JPEGs are decoded on the GPU; anything else, and any
-    JPEG whose stream the decoder reports malformed, by Pillow, whose exceptions propagate."""
-    dev = torch.device(device)
-    if dev.type != "cuda":
-        raise RuntimeError(f"must3r_b200 JPEG decoding runs on CUDA devices only (got device {dev})")
-    if dev.index is None:
-        dev = torch.device("cuda", torch.cuda.current_device())
-    return decode_parsed_all([Parsed(p, exif_transpose) for p in paths], dev)
+    """engine.imagefiles.decode_files: one CUDA uint8 [H,W,3] tensor per path, bitwise equal to
+    np.asarray(PIL.Image.open(p).convert('RGB')) (after PIL.ImageOps.exif_transpose when `exif_transpose`), eligible
+    JPEGs and PNGs decoded on the GPU, anything else by Pillow, whose exceptions propagate."""
+    from . import imagefiles
+    return imagefiles.decode_files(paths, device, exif_transpose)

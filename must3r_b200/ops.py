@@ -559,3 +559,37 @@ def jpeg_decode(descs, dev_blob: torch.Tensor, descs_off: int, work: torch.Tenso
     assert status.dtype == torch.int32 and status.numel() >= len(descs)
     _lib.check(_lib.lib().m3r_jpeg_decode(descs, len(descs), _p(dev_blob), descs_off, _p(work), work.numel(), _p(status),
                                           _stream()), "jpeg_decode")
+
+
+# ------------------------------------------------------------------------------------------- PNG decoding
+def png_parse(data: bytes) -> "_lib.PngInfo":
+    """Chunk facts of a PNG held in memory (m3r_png_parse); info.eligible says whether png_decode takes it.  A file that
+    is not a PNG comes back with eligible == 0."""
+    info = _lib.PngInfo()
+    _lib.lib().m3r_png_parse(data, len(data), C.byref(info))
+    return info
+
+
+def png_prepare(data: bytes, info, orientation: int, dst_ptr: int, base_off: int) -> "_lib.PngDesc":
+    """Palette and concatenated IDAT payloads of one eligible image written at host address dst_ptr (info.prep_bytes
+    bytes); its descriptor."""
+    desc = _lib.PngDesc()
+    _lib.check(_lib.lib().m3r_png_prepare(data, len(data), C.byref(info), orientation, C.c_void_p(dst_ptr), base_off,
+                                          C.byref(desc)), "png_prepare")
+    return desc
+
+
+def png_plan(descs) -> int:
+    """Fill the workspace fields of a ctypes array of PngDesc; returns the workspace bytes png_decode needs."""
+    n = _lib.lib().m3r_png_plan(descs, len(descs))
+    if n < 0:
+        _lib.check(1, "png_plan")
+    return n
+
+
+def png_decode(descs, dev_blob: torch.Tensor, descs_off: int, work: torch.Tensor, status: torch.Tensor) -> None:
+    """Decode a planned batch on the current stream; status [n] int32 gets each image's M3R_PNG_E* bits."""
+    _req_cuda(dev_blob, work, status)
+    assert status.dtype == torch.int32 and status.numel() >= len(descs)
+    _lib.check(_lib.lib().m3r_png_decode(descs, len(descs), _p(dev_blob), descs_off, _p(work), work.numel(), _p(status),
+                                         _stream()), "png_decode")
