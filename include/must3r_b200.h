@@ -20,7 +20,7 @@
 extern "C" {
 #endif
 
-#define M3R_ABI_VERSION 4
+#define M3R_ABI_VERSION 5
 #define M3R_MAX_PEERS 8
 #define M3R_MAX_GROUPS 16
 
@@ -630,7 +630,7 @@ int m3r_decoder_forward(const m3r_decoder_weights* w, const m3r_decoder_call* ca
  * int32 device array [B] (values clamped to [0, call->Nm]); call->Nm is the longest memory and must be >= 1, and each
  * scene's memory rows begin at b * mem_bstride_rows.  Every layer's memory cross-attention runs as m3r_attention_ragged.
  * Only memory_mode kv with new_only = 1 (no render, no peers, no context parallel): the new post-feedback K|V rows of
- * every scene go to mem_out[l] [B, Nt, 2D] and nothing is written into the memory; m3r_mem_commit appends them.  The
+ * every scene go to mem_out[l] [B, Nt, 2D] and nothing is written into the memory; m3r_mem_commit_rows appends them.  The
  * workspace is m3r_decoder_workspace_bytes(w, call). */
 int m3r_decoder_forward_ragged(const m3r_decoder_weights* w, const m3r_decoder_call* call, const int32_t* nm_scene,
                                void* workspace, int64_t workspace_bytes, void* stream);
@@ -662,19 +662,14 @@ int m3r_decoder_forward_e4m3(const m3r_decoder_weights* w, const m3r_decoder_e4m
 int m3r_decoder_render_ragged(const m3r_decoder_weights* w, const m3r_decoder_e4m3* w8, const m3r_decoder_call* call,
                               const int32_t* nm_scene, void* workspace, int64_t workspace_bytes, void* stream);
 
-/* Keyframe commit of several SLAM sessions in one launch: for each scene b < B whose flag keep[b * keep_stride] (int32,
- * device; e.g. the keyframe field of its m3r_slam_record) is non-zero, copy rows [0, Nt) of staged[l] + b * Nt * width
- * (the [B, Nt, width] 16-bit new_only output of m3r_decoder_forward_ragged) to rows dst_row[b] .. dst_row[b] + Nt - 1 of
- * arena[l] (rows of `width` 16-bit elements), for every level l < depth.  A scene whose flag is zero writes nothing.
- * arena, staged: host arrays [depth] of device pointers; dst_row: host array [B].  B <= M3R_MAX_COMMIT,
- * depth <= M3R_MAX_GROUPS, width % 8 == 0, every arena / staged pointer 16-byte aligned and keep 4-byte aligned. */
+/* Memory commit of B scenes in one launch: scene b < B whose flag keep[b * keep_stride] (int32, device; e.g. the keyframe
+ * field of its m3r_slam_record) is non-zero copies rows [row0, row0 + rows) of staged[l] + b * src_stride_rows * width
+ * (e.g. the [B, Nt, width] 16-bit new_only output of m3r_decoder_forward_ragged) to rows dst_row[b] .. dst_row[b] + rows - 1
+ * of arena[l] (rows of `width` 16-bit elements), for every level l < depth; a refinement pass skips the reference view's
+ * rows with row0 > 0.  arena, staged: host arrays [depth] of device pointers; dst_row: host array [B].  B <= M3R_MAX_COMMIT,
+ * depth <= M3R_MAX_GROUPS, width % 8 == 0, 0 <= row0, row0 + rows <= src_stride_rows, every arena / staged pointer
+ * 16-byte aligned and keep 4-byte aligned. */
 #define M3R_MAX_COMMIT 64
-int m3r_mem_commit(void* const* arena, const void* const* staged, int32_t depth, int32_t B, int32_t Nt, int32_t width,
-                   const int64_t* dst_row, const int32_t* keep, int64_t keep_stride, void* stream);
-/* m3r_mem_commit of part of each staged block: rows [row0, row0 + rows) of staged[l] + b * src_stride_rows * width go to
- * rows dst_row[b] .. dst_row[b] + rows - 1 of arena[l].  m3r_mem_commit is the case row0 = 0, rows = src_stride_rows = Nt.
- * Used where a refinement pass overwrites a step's rows in place except those of the reference view.  Same conditions,
- * and 0 <= row0, row0 + rows <= src_stride_rows. */
 int m3r_mem_commit_rows(void* const* arena, const void* const* staged, int32_t depth, int32_t B, int32_t row0, int32_t rows,
                         int32_t src_stride_rows, int32_t width, const int64_t* dst_row, const int32_t* keep,
                         int64_t keep_stride, void* stream);
@@ -682,7 +677,7 @@ int m3r_mem_commit_rows(void* const* arena, const void* const* staged, int32_t d
  * shared memory (must3r_b200/engine/slam_cameras.py): frame k < F whose flag keep[k * keep_stride] (int32, device; the
  * keyframe field of its m3r_slam_record) is non-zero copies rows [0, Nt) of staged[l] + k * Nt * width (the [F, Nt, width]
  * 16-bit new_only output of the decoder) to rows row0 + Nt * j .. row0 + Nt * (j + 1) - 1 of arena[l], j being the number
- * of frames before k whose flag is set, for every level l < depth.  The result is bitwise that of m3r_mem_commit called
+ * of frames before k whose flag is set, for every level l < depth.  The result is bitwise that of m3r_mem_commit_rows called
  * frame after frame with the rows counted on the host; rows past row0 + Nt * (flags set) are not written.  The flags are
  * read on the device.  arena, staged: host arrays [depth] of device pointers.  F <= M3R_MAX_COMMIT,
  * depth <= M3R_MAX_GROUPS, width % 8 == 0, row0 >= 0, every arena / staged pointer 16-byte aligned, keep 4-byte aligned. */

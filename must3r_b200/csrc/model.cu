@@ -734,11 +734,6 @@ static int mem_commit(void* const* arena, const void* const* staged, int32_t dep
   return 0;
 }
 
-extern "C" int m3r_mem_commit(void* const* arena, const void* const* staged, int32_t depth, int32_t B, int32_t Nt, int32_t width,
-                              const int64_t* dst_row, const int32_t* keep, int64_t keep_stride, void* stream) {
-  return mem_commit(arena, staged, depth, B, 0, Nt, Nt, width, dst_row, keep, keep_stride, stream);
-}
-
 extern "C" int m3r_mem_commit_rows(void* const* arena, const void* const* staged, int32_t depth, int32_t B, int32_t row0,
                                    int32_t rows, int32_t src_stride_rows, int32_t width, const int64_t* dst_row,
                                    const int32_t* keep, int64_t keep_stride, void* stream) {

@@ -8,11 +8,11 @@ is_sequence=True)` returns for that list alone, but the scenes share their calls
     (demo._mem_batches) and views to render (demo._to_render), its steps' views grouped by shape and cut at `max_bs` as
     inference_multi_ar does (stack_views).
   * The views of all scenes are encoded up front, grouped by shape, up to ENCODE_AHEAD_BATCH views per call.
-  * The memories live in one SessionArena (engine/slam_sessions.py), one slot per scene, sized once for the schedule.
+  * The memories live in one SessionArena (engine/lockstep.py), one slot per scene, sized once for the schedule.
   * Step k of every scene that has one runs in the same decoder calls: the scenes whose step views have the same shapes
-    share a call (plan_batch's rule, then one call per run of consecutive slots, slot_runs).  A step is one
-    MUSt3R.update_tokens call (the first one without a memory; every later one with the scenes' memory lengths, so each
-    scene attends only to its own rows) followed by one m3r_mem_commit_rows that writes the new rows into the slots.
+    share a call (lockstep_calls).  A step is its MUSt3R.update_tokens calls (the first step's without a memory; every
+    later one with the scenes' memory lengths, so each scene attends only to its own rows), then the commit of every
+    scene's new rows into its slot (ScenePlan.step's edit, lockstep.apply_edits).
   * A refinement pass re-runs every step against the full memories and overwrites each step's rows in place, except those
     of the reference view (label 0: the first view of the first step), as inference_multi_ar's refresh branch does.
   * The render pass runs in chunks of up to `max_bs` views per scene (MUSt3R.render_tokens, m3r_decoder_render_ragged);
@@ -29,39 +29,18 @@ memory-batch loop never ends).
 """
 from __future__ import annotations
 
-import ctypes as C
 import datetime
+import itertools
 from typing import List, Sequence
 
 import torch
 
-from .. import _lib
 from ..model import get_pointmaps_activation
-from ..model import common as cm
 from .demo import (SceneState, _amp, _finish_scene, _launch_scene_copies, _linspace_keyframes, _load, _mem_batches,
                    _report, _to_render)
-from .inference import ENCODE_AHEAD_BATCH, _sync_host_copies, postprocess, stack_views
-from .slam_sessions import SessionArena, plan_batch, slot_runs
-
-MAX_COMMIT = 64         # M3R_MAX_COMMIT: scenes per m3r_mem_commit_rows launch
-
-
-def _tokens(hw):
-    return (hw[0] // 16) * (hw[1] // 16)
-
-
-def _groups(shapes, positions, max_bs):
-    """stack_views' grouping of the views at `positions` (by shape, lexicographic, cut at max_bs) -> [((H, W), [pos])]."""
-    if not positions:
-        return []
-    ts = torch.tensor([shapes[p] for p in positions], dtype=torch.int32).view(-1, 2)
-    _, idx_st = stack_views(ts, [], max_bs=max_bs)
-    return [(shapes[positions[idx[0]]], [positions[i] for i in idx]) for idx in idx_st]
-
-
-def signature(groups):
-    """What scenes must share to run a step or render chunk in one call: the shape and view count of every group."""
-    return tuple((hw, len(pos)) for hw, pos in groups)
+from .inference import _sync_host_copies, postprocess
+from .lockstep import (SessionArena, StepEdit, _call_inputs, _encode, _groups, _tokens, apply_edits, lockstep_calls,
+                       signature)
 
 
 class ScenePlan:
@@ -101,17 +80,13 @@ class ScenePlan:
         of step 0's first group) are never overwritten."""
         return _tokens(self.steps[0][0][0]) if step == 0 else 0
 
-
-def lockstep_calls(items):
-    """items [(slot, signature)] in slot order -> [(signature, [slots])]: the scenes of the most common signature first
-    (plan_batch; the first such signature on a tie), each cut into runs of consecutive slots; then the rest likewise."""
-    cands = dict(items)
-    calls = []
-    while cands:
-        batch, rest = plan_batch(cands)
-        calls += [(cands[batch[0]], run) for run in slot_runs(batch)]
-        cands = {s: cands[s] for s in rest}
-    return calls
+    def step(self, it, k) -> StepEdit:
+        """The memory edit after step k of pass `it`: pass 0 writes the step's rows behind the memory, a refinement pass
+        overwrites them in place from refresh_row0(k) on."""
+        rows = sum(_tokens(hw) * len(pos) for hw, pos in self.steps[k])
+        row0 = self.refresh_row0(k) if it else 0
+        length = self.mem_rows if it else self.step_start[k] + rows
+        return StepEdit([], (row0, self.step_start[k] + row0, rows - row0), length)
 
 
 def plan_memory_calls(plans: List[ScenePlan], num_refinements_iterations=0):
@@ -136,56 +111,6 @@ def plan_render_calls(plans: List[ScenePlan]):
 def arena_rows(plans: List[ScenePlan]):
     """Rows per slot of the scenes' arena: the largest memory of the schedule (refinement passes stage their rows apart)."""
     return max(p.mem_rows for p in plans)
-
-
-def _host_shape(hw, B, n):
-    ts = torch.tensor(hw, dtype=torch.int32).view(1, 1, 2).expand(B, n, 2)
-    ts._m3r_hw = tuple(hw)          # the decoder reads (H, W) from here: no device read
-    return ts
-
-
-def _commit_rows(arena, staged, slots, row0, rows, dst_rows, keep, stream):
-    """m3r_mem_commit_rows of staged rows [row0, row0 + rows) of each scene to its slot at dst_rows[b]."""
-    lib = _lib.lib()
-    depth = arena.depth
-    bufs = (C.c_void_p * depth)(*[b.data_ptr() for b in arena.bufs])
-    Nt = staged[0].shape[1]
-    for lo in range(0, len(slots), MAX_COMMIT):
-        hi = min(lo + MAX_COMMIT, len(slots))
-        src = (C.c_void_p * depth)(*[t[lo].data_ptr() for t in staged])
-        dst = (C.c_int64 * (hi - lo))(*[slots[b] * arena.cap + dst_rows[b] for b in range(lo, hi)])
-        _lib.check(lib.m3r_mem_commit_rows(bufs, src, depth, hi - lo, row0, rows, Nt, arena.width, dst,
-                                           C.c_void_p(keep.data_ptr()), 0, stream), "mem_commit_rows")
-
-
-def _encode(encoder, plans, imgs, device, max_bs):
-    """Every view of every scene, grouped by shape -> feats[s][position] = (x [N, D], pos [N, 2])."""
-    S = len(plans)
-    bs = ENCODE_AHEAD_BATCH if max_bs is None else min(ENCODE_AHEAD_BATCH, max_bs * S)
-    by_shape = {}
-    for s, p in enumerate(plans):
-        for q, hw in enumerate(p.shapes):
-            by_shape.setdefault(hw, []).append((s, q))
-    feats = [[None] * len(p.order) for p in plans]
-    for hw, members in by_shape.items():
-        for lo in range(0, len(members), bs):
-            chunk = members[lo:lo + bs]
-            ts = torch.tensor([hw] * len(chunk), dtype=torch.int32)       # host: the encoder reads it there
-            xs, ps = encoder(torch.stack([imgs[s][q] for s, q in chunk]).to(device), ts)
-            for j, (s, q) in enumerate(chunk):
-                feats[s][q] = (xs[j], ps[j])
-    return feats
-
-
-def _call_inputs(feats, plans, run, groups_of):
-    """Stacked decoder inputs of one call: per group x [B, n, N, D], pos [B, n, N, 2], true_shape [B, n, 2]."""
-    xs, ps, ts = [], [], []
-    for g, (hw, _) in enumerate(groups_of(plans[run[0]])):
-        members = [groups_of(plans[s])[g][1] for s in run]
-        xs.append(torch.stack([torch.stack([feats[s][q][0] for q in pos]) for s, pos in zip(run, members)]))
-        ps.append(torch.stack([torch.stack([feats[s][q][1] for q in pos]) for s, pos in zip(run, members)]))
-        ts.append(_host_shape(hw, len(run), len(members[0])))
-    return xs, ps, ts
 
 
 @torch.no_grad()
@@ -234,35 +159,29 @@ def _run(encoder, decoder, plans, imgs, device, act, max_bs, num_refinements_ite
     _phase("memory")
     arena = SessionArena(S, decoder.depth, 2 * decoder.embed_dim, decoder.memory_dtype(), dev)
     arena.ensure(arena_rows(plans))
-    keep = torch.ones(1, dtype=torch.int32, device=dev)
-    stream = cm.stream_ptr(dev)
     pending = []          # (H, W), raw pointmaps [rows, H, W, 7], [(slot, position)] per row, 0: memory step / 1: render
 
-    for it, step, sig, run in plan_memory_calls(plans, num_refinements_iterations):
-        xs, ps, ts = _call_inputs(feats, plans, run, lambda p: p.steps[step])
-        if it == 0 and step == 0:
-            new, pms = decoder.update_tokens(xs, ps, ts, current_mem=None)
-        else:
-            mem = ([b[run[0]:run[-1] + 1] for b in arena.bufs], None, 0, 0, 0)
-            new, pms = decoder.update_tokens(xs, ps, ts, current_mem=mem, mem_lengths=[arena.lengths[s] for s in run])
-        Nt = new[0].shape[1]
-        row0 = 0 if it == 0 else plans[run[0]].refresh_row0(step)
-        _commit_rows(arena, new, run, row0, Nt - row0, [plans[s].step_start[step] + row0 for s in run], keep, stream)
-        if it == 0:
-            for s in run:
-                assert arena.lengths[s] == plans[s].step_start[step]
-                arena.lengths[s] += Nt
-        if it == num_refinements_iterations and plans[run[0]].first_positions:       # render_once: returned as they are
-            for g, pm in enumerate(pms):
-                members = [(s, q) for s in run for q in plans[s].steps[step][g][1]]
-                pending.append((sig[g][0], pm.flatten(0, 1), members, 0))
+    for (it, step), calls in itertools.groupby(plan_memory_calls(plans, num_refinements_iterations), lambda c: c[:2]):
+        staged = []       # the calls of a step touch disjoint slots: their rows are committed after the last one
+        for _, _, sig, run in calls:
+            xs, ps, ts = _call_inputs(feats, plans, run, lambda p: p.steps[step])
+            if it == 0 and step == 0:
+                new, pms = decoder.update_tokens(xs, ps, ts, current_mem=None)
+            else:
+                new, pms = decoder.update_tokens(xs, ps, ts, current_mem=arena.memory(run),
+                                                 mem_lengths=[arena.lengths[s] for s in run])
+            staged.append((run, new))
+            if it == num_refinements_iterations and plans[run[0]].first_positions:   # render_once: returned as they are
+                for g, pm in enumerate(pms):
+                    members = [(s, q) for s in run for q in plans[s].steps[step][g][1]]
+                    pending.append((sig[g][0], pm.flatten(0, 1), members, 0))
+        apply_edits(arena, staged, {s: plans[s].step(it, step) for run, _ in staged for s in run})
 
     _phase("render")
     if any(p.render for p in plans):
         for c, sig, run in plan_render_calls(plans):
             (xs,), (ps,), (ts,) = _call_inputs(feats, plans, run, lambda p: [p.render[c]])
-            mem = ([b[run[0]:run[-1] + 1] for b in arena.bufs], None, 0, 0, 0)
-            pm = decoder.render_tokens(xs, ps, ts, mem, [arena.lengths[s] for s in run])
+            pm = decoder.render_tokens(xs, ps, ts, arena.memory(run), [arena.lengths[s] for s in run])
             pending.append((sig[0][0], pm.flatten(0, 1), [(s, q) for s in run for q in plans[s].render[c][1]], 1))
 
     _phase("postprocess")

@@ -13,7 +13,7 @@ maps (keep_memory) are kept in the same order.  With one camera this is SLAM_MUS
 difference from the reference is that a frame does not see a keyframe taken earlier in the same step: two cameras that
 look at new ground at the same instant may both become keyframes where the reference would take only the first.
 
-Batching rule (plan_batch of engine/slam_sessions.py): the step's frames are batched when the memory is non-empty, the
+Batching rule (plan_batch of engine/lockstep.py): the step's frames are batched when the memory is non-empty, the
 run is past the initialisation re-runs (`num_init_frames`, after a fresh start or load_memory), the decoder keeps its
 memory as K|V rows (memory_mode 'kv'), and a frame's preprocessed shape is the shape most frames of the step share.  The
 batch costs one encoder call, one decoder call in which the F frames read the one memory through a stride-0 scene
@@ -27,29 +27,26 @@ keyframe was taken.  Every other frame (another preprocessed shape in a step tha
 SLAM_MUSt3R.__call__ after the batch, in camera order: its timestamp, pose and keyframe are recorded after the batch's,
 and it sees the batch's keyframes.
 
-Memory: one [1, cap, 2D] buffer per level (SessionArena of engine/slam_sessions.py with one slot), grown geometrically
+Memory: one [1, cap, 2D] buffer per level (SessionArena of engine/lockstep.py with one slot), grown geometrically
 before a step that could overflow it; the run's `memory` is the reference's 5-tuple of views of it, so save_memory,
 pickling and load_memory work unchanged.
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import Dict
 
 import numpy as np
 import torch
 
-from .. import _lib, ops
+from .. import ops
 from ..model import get_pointmaps_activation
-from ..model import common as cm
 from . import slam
 from .images import preproc_frame
 from .inference import _to_out, postprocess
 from .keyframes import QuadrantSearcher, get_quadrant_id
 from .slam import SLAM_MUSt3R, _index_ready, mean_focal, prep_imgs
-from .slam_sessions import KEYFRAME_OFFSET, SLAMSessions, plan_batch
-
-MAX_CAMERAS = 64         # M3R_MAX_COMMIT: frames per m3r_mem_commit_ordered launch
+from .lockstep import MAX_COMMIT, commit_ordered, plan_batch
+from .slam_sessions import KEYFRAME_FIELD, SLAMSessions
 
 
 def steps_of(items):
@@ -91,8 +88,8 @@ class MultiCameraSLAM(SLAMSessions):
     SLAM_MUSt3R's."""
 
     def __init__(self, chkpt, num_cameras=1, device='cuda:0', **kwargs):
-        if not 1 <= num_cameras <= MAX_CAMERAS:
-            raise ValueError(f"num_cameras must be in [1, {MAX_CAMERAS}]")
+        if not 1 <= num_cameras <= MAX_COMMIT:             # the frames of a step go to one m3r_mem_commit_ordered
+            raise ValueError(f"num_cameras must be in [1, {MAX_COMMIT}]")
         if kwargs.get('rerender') and num_cameras > 1:
             raise ValueError("rerendering with several cameras (different focal lengths) is not supported")
         super().__init__(chkpt, 1, device=device, num_agents=num_cameras, **kwargs)
@@ -155,16 +152,6 @@ class MultiCameraSLAM(SLAMSessions):
         new_tokens, pm = decoder.update_tokens(x[:, None], pos[:, None], shape, current_mem=mem)
         return postprocess(pm, pointmaps_activation=get_pointmaps_activation(decoder, verbose=False)), new_tokens
 
-    def _commit_ordered(self, new_tokens, recs):
-        """m3r_mem_commit_ordered: the rows of the frames whose record says keyframe, behind the memory in batch order."""
-        depth = self.arena.depth
-        arena = (C.c_void_p * depth)(*[b.data_ptr() for b in self.arena.bufs])
-        src = (C.c_void_p * depth)(*[t.data_ptr() for t in new_tokens])
-        F, N = new_tokens[0].shape[:2]
-        _lib.check(_lib.lib().m3r_mem_commit_ordered(arena, src, depth, F, N, self.arena.width, self.arena.lengths[0],
-                                                     C.c_void_p(recs.data_ptr() + KEYFRAME_OFFSET), recs.shape[1] // 4,
-                                                     cm.stream_ptr(recs.device)), "mem_commit_ordered")
-
     def _launch_tails(self, batch, res, prepped, recs):
         """The device half of the agents' `update` for the F frames of the batch at once, which never waits: one
         m3r_slam_pose_views with each camera's focal, one searcher query over all frames' subsampled points, one
@@ -197,7 +184,8 @@ class MultiCameraSLAM(SLAMSessions):
         recs = torch.empty((len(batch), ops.SLAM_RECORD.itemsize), dtype=torch.uint8, device=torch.device(self.device))
         preds = [{k: res[k][i:i + 1] for k in ('pts3d', 'pts3d_local', 'conf')} for i in range(len(batch))]
         tails = self._launch_tails(batch, res, prepped, recs)
-        self._commit_ordered(new_tokens, recs)
+        flags = recs.view(torch.int32)[:, KEYFRAME_FIELD]
+        commit_ordered(self.arena, new_tokens, flags, flags.stride(0))
         host_recs = _to_out(recs, 'cpu')
         slam._wait_host_copies()
         records = host_recs.numpy().view(ops.SLAM_RECORD)[:, 0]

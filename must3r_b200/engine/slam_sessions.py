@@ -10,103 +10,33 @@ rows (memory_mode 'kv'), and its preprocessed shape is the batch's shape (the sh
 batch then costs one encoder call over its frames, one decoder call in which each frame attends only to its own
 session's memory (MUSt3R.update_tokens with mem_lengths, csrc/model.cu m3r_decoder_forward_ragged), the per-session
 pose, searcher query and keyframe kernels (MUSt3R_Agent.launch_tail, each into its row of one batch of records), one
-m3r_mem_commit that appends the new rows of the sessions whose frame is a keyframe, and one wait for all records and
-returned arrays (engine/slam.py's _wait_host_copies); then each frame finishes as in SLAM_MUSt3R.__call__
+commit (lockstep.commit) that appends the new rows of the sessions whose frame is a keyframe, and one wait for all
+records and returned arrays (engine/slam.py's _wait_host_copies); then each frame finishes as in SLAM_MUSt3R.__call__
 (MUSt3R_Agent.finish_tail, SLAM_MUSt3R._record_frame).  Every other frame runs alone through SLAM_MUSt3R.__call__ and its
 resulting memory is copied into its session's slot.
 
-Memory: per decoder level one arena [S, cap, 2D] (SessionArena); session s's memory is rows [0, n_s) of slot s.  The
-arena grows geometrically, for all sessions with one copy per level, when a session would overflow.  Each session's
-`memory` is the reference's 5-tuple whose tensors are views of its slot, so save_memory, pickling and load_memory work
-unchanged.
+Memory: per decoder level one arena [S, cap, 2D] (SessionArena of engine/lockstep.py); session s's memory is rows
+[0, n_s) of slot s.  The arena grows geometrically, for all sessions with one copy per level, when a session would
+overflow.  Each session's `memory` is the reference's 5-tuple whose tensors are views of its slot, so save_memory,
+pickling and load_memory work unchanged.
 """
 from __future__ import annotations
 
-import ctypes as C
-import math
 from collections import Counter
-from typing import Dict, List, Optional, Sequence
+from typing import Dict
 
 import numpy as np
 import torch
 
-from .. import _lib, ops
+from .. import ops
 from ..model import get_pointmaps_activation, load_model
-from ..model import common as cm
 from . import slam
 from .images import preproc_frame
 from .inference import _reserve, _to_out, postprocess
+from .lockstep import SessionArena, commit, plan_batch, slot_runs
 from .slam import SLAM_MUSt3R
 
-KEYFRAME_OFFSET = ops.SLAM_RECORD.fields["keyframe"][1]        # byte offset of the keyframe flag in a record
-
-
-class SessionArena:
-    """Per level one [S, cap, width] buffer; slot s holds session s's memory rows [0, lengths[s]).  `ensure(rows)` grows
-    every level geometrically (by `growth`, at least to `rows`) with one copy of the used rows for all sessions."""
-
-    def __init__(self, S, depth, width, dtype, device, growth=1.5, min_cap=0):
-        self.S, self.depth, self.width, self.dtype, self.device = S, depth, width, dtype, torch.device(device)
-        self.growth, self.min_cap = growth, min_cap
-        self.cap = 0
-        self.bufs: List[torch.Tensor] = []
-        self.lengths = [0] * S
-
-    def ensure(self, rows):
-        """Room for `rows` rows in every slot; True if the buffers were reallocated (views handed out before stay valid,
-        on the old buffers)."""
-        if rows <= self.cap:
-            return False
-        cap = max(rows, int(math.ceil(self.cap * self.growth)), self.min_cap)
-        used = max(self.lengths)
-        new = [torch.empty((self.S, cap, self.width), dtype=self.dtype, device=self.device) for _ in range(self.depth)]
-        for n, o in zip(new, self.bufs):
-            if used:
-                n[:, :used].copy_(o[:, :used])
-        self.bufs, self.cap = new, cap
-        return True
-
-    def views(self, s, rows=None):
-        rows = self.lengths[s] if rows is None else rows
-        return [b[s:s + 1, :rows] for b in self.bufs]
-
-    def holds(self, s, mem_vals):
-        """True if mem_vals are already the views of slot s (nothing to copy)."""
-        return (len(self.bufs) == len(mem_vals) and mem_vals[0].shape[1] == self.lengths[s]
-                and all(m.data_ptr() == b[s].data_ptr() for m, b in zip(mem_vals, self.bufs)))
-
-    def store(self, s, mem_vals):
-        """Copy a [1, n, width] memory (list per level) into slot s."""
-        n = mem_vals[0].shape[1]
-        self.ensure(n)
-        for b, m in zip(self.bufs, mem_vals):
-            b[s, :n].copy_(m[0])
-        self.lengths[s] = n
-
-
-def plan_batch(cands: Dict[int, Optional[tuple]]):
-    """The batching rule.  cands: session id -> its frame's preprocessed (H, W), or None when the frame must run alone
-    (empty memory, an initialisation re-run, a memory_mode other than 'kv').  -> (batched ids, alone ids), both in the
-    order given.  The batch takes the shape most frames share (the first such shape on a tie).  A batch of one frame
-    still takes the batched path: its memory stays in its slot, where the single-session path would copy it there."""
-    shapes = Counter(sh for sh in cands.values() if sh is not None)
-    if not shapes:
-        return [], list(cands)
-    best = max(shapes.values())
-    shape = next(sh for sh in cands.values() if sh is not None and shapes[sh] == best)
-    batch = [sid for sid, sh in cands.items() if sh == shape]
-    return batch, [sid for sid in cands if sid not in batch]
-
-
-def slot_runs(slots: Sequence[int]):
-    """Sorted slot indices -> runs of consecutive slots (one decoder call each: its scenes must be evenly strided)."""
-    runs = []
-    for s in slots:
-        if runs and s == runs[-1][-1] + 1:
-            runs[-1].append(s)
-        else:
-            runs.append([s])
-    return runs
+KEYFRAME_FIELD = ops.SLAM_RECORD.fields["keyframe"][1] // 4     # int32 index of the keyframe flag in a record
 
 
 class _Session(SLAM_MUSt3R):
@@ -213,10 +143,9 @@ class SLAMSessions:
             i1 = i0 + len(run)
             shape = ts[i0:i1].view(i1 - i0, 1, 2)
             shape._m3r_hw = hw
-            mem = ([b[run[0]:run[-1] + 1] for b in self.arena.bufs], None, 0, 0, 0)
             lengths = [self.arena.lengths[sl] for sl in run]
-            new_tokens, pm = decoder.update_tokens(x[i0:i1, None], pos[i0:i1, None], shape, current_mem=mem,
-                                                   mem_lengths=lengths)
+            new_tokens, pm = decoder.update_tokens(x[i0:i1, None], pos[i0:i1, None], shape,
+                                                   current_mem=self.arena.memory(run), mem_lengths=lengths)
             staged.append((batch[i0:i1], new_tokens))
             pms.append(pm)
             i0 = i1
@@ -224,19 +153,14 @@ class SLAMSessions:
         return postprocess(pm, pointmaps_activation=act), staged
 
     def _commit(self, staged, recs, index):
-        """m3r_mem_commit of each run: the new rows of the sessions whose record says keyframe, behind their memory."""
-        lib = _lib.lib()
-        depth = self.arena.depth
-        arena = (C.c_void_p * depth)(*[b.data_ptr() for b in self.arena.bufs])
+        """Each run's new rows of the sessions whose record says keyframe, behind their memory."""
+        flags = recs.view(torch.int32)[:, KEYFRAME_FIELD]
         for members, new_tokens in staged:
             i0 = index[members[0]]
             assert [index[m] for m in members] == list(range(i0, i0 + len(members)))
-            src = (C.c_void_p * depth)(*[t.data_ptr() for t in new_tokens])
-            rows = (C.c_int64 * len(members))(*[self.sessions[m].slot * self.arena.cap + self.arena.lengths[self.sessions[m].slot]
-                                                for m in members])
-            keep = recs.data_ptr() + i0 * recs.shape[1] + KEYFRAME_OFFSET
-            _lib.check(lib.m3r_mem_commit(arena, src, depth, len(members), new_tokens[0].shape[1], self.arena.width, rows,
-                                          C.c_void_p(keep), recs.shape[1] // 4, cm.stream_ptr(recs.device)), "mem_commit")
+            slots = [self.sessions[m].slot for m in members]
+            commit(self.arena, new_tokens, slots, [self.arena.lengths[s] for s in slots], keep=flags[i0:],
+                   keep_stride=flags.stride(0))
 
     def _step_batch(self, batch, frames, prepped):
         dev = torch.device(self.device)

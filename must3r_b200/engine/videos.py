@@ -5,11 +5,11 @@ list, the SceneState that `demo.get_reconstructed_scene(..., execution_mode=...)
 (must3r_inference_video with init_num_images=2, batch_num_views=1 and the mode's keyframe test), but the scenes share
 their calls:
 
-  * All frames of all scenes are encoded up front, grouped by shape (scenes._encode).
+  * All frames of all scenes are encoded up front, grouped by shape (lockstep._encode).
   * Step k of every scene that has one runs in shared decoder calls: the scenes whose step views have the same shapes
-    share a call, cut into runs of consecutive slots (scenes.lockstep_calls).  Step 0 (the init views) is one
+    share a call, cut into runs of consecutive slots (lockstep_calls).  Step 0 (the init views) is one
     MUSt3R.update_tokens call without a memory; every later step passes the scenes' memory lengths, so each scene attends
-    only to its own rows.  The memories live in one SessionArena, one slot per scene.
+    only to its own rows.  The memories live in one SessionArena (engine/lockstep.py), one slot per scene.
   * Keyframes: vidseq's test (id % keyframe_interval == 0) is known on the host, so the frame loop waits for nothing and
     the arena is sized once.  vidslam postprocesses each step's frames together; every scene's searcher query and
     m3r_slam_keyframe fill one row of one record tensor, read back with one wait per step whatever the number of scenes;
@@ -20,6 +20,7 @@ their calls:
     (m3r_mem_commit_rows): behind the scene's memory, or over a keyframe's old rows in a refinement pass (except those of
     the reference view, label 0).  A frame that leaves the window right after its own step (local_context_size=0, not a
     keyframe) is never written.  Between passes only keyframes stay; after the last pass nothing is compacted.
+    lockstep.apply_edits applies every scene's StepEdit.
   * Results are those of the last pass.  postprocess(compute_cam=True) runs once per step and view group over all the
     scenes' frames (vidseq: after the frame loop), and every scene's results are copied to the host in one batch of
     asynchronous copies followed by one wait.
@@ -30,35 +31,24 @@ Only memory_mode 'kv' is supported.
 from __future__ import annotations
 
 import copy
-import ctypes as C
 import datetime
 from collections import deque
-from typing import List, NamedTuple, Optional
+from typing import List
 
 import numpy as np
 import torch
 
-from .. import _lib, ops
+from .. import ops
 from ..model import get_pointmaps_activation
-from ..model import common as cm
 from .demo import (SceneState, _amp, _finish_scene, _launch_scene_copies, _load, _mem_batches, _report,
                    slam_update_scene_state)
 from .inference import _sync_host_copies, _to_out, postprocess
 from .keyframes import choose_keyframe_from_overlap, get_searcher
-from .scenes import MAX_COMMIT, _call_inputs, _commit_rows, _encode, _groups, _tokens, lockstep_calls, signature
-from .slam_sessions import SessionArena
+from .lockstep import (SessionArena, StepEdit, _call_inputs, _encode, _groups, _tokens, apply_edits, lockstep_calls,
+                       signature)
 
-MAX_COMPACT_RUNS = 128          # M3R_MAX_COMPACT_RUNS: runs per m3r_mem_compact_rows launch
 OVERLAP_MODE = "nn-norm"        # demo.get_reconstructed_scene's vidslam overlap score
 SEARCHER = "kdtree-scipy-quadrant_x2"
-
-
-class StepEdit(NamedTuple):
-    """One scene's memory edit after one step, in rows of its slot.  runs: the compaction [(src_row, dst_row, rows)],
-    applied first; write: (staged_row, dst_row, rows), the step's new rows that stay, or None; length: rows afterwards."""
-    runs: list
-    write: Optional[tuple]
-    length: int
 
 
 def _find(blocks, label):
@@ -186,56 +176,8 @@ class VideoPlan:
 
 
 def plan_step_calls(plans: List[VideoPlan], k):
-    """The lockstep calls of step k -> [(signature, [slots])] (scenes.lockstep_calls)."""
+    """The lockstep calls of step k -> [(signature, [slots])] (lockstep_calls)."""
     return lockstep_calls([(s, signature(p.steps[k])) for s, p in enumerate(plans) if k < len(p.steps)])
-
-
-def _compact_rows(arena, runs_of, stream):
-    """m3r_mem_compact_rows of {slot: runs}, in launches of at most MAX_COMMIT scenes and MAX_COMPACT_RUNS runs (a scene
-    whose runs do not fit goes on in the next launch: applied in order, runs compose)."""
-    lib = _lib.lib()
-    depth = arena.depth
-    bufs = (C.c_void_p * depth)(*[b.data_ptr() for b in arena.bufs])
-    launches, cur, n = [], [], 0
-    for slot in sorted(runs_of):
-        runs = list(runs_of[slot])
-        while runs:
-            if n == MAX_COMPACT_RUNS or len(cur) == MAX_COMMIT:
-                launches.append(cur)
-                cur, n = [], 0
-            take, runs = runs[:MAX_COMPACT_RUNS - n], runs[MAX_COMPACT_RUNS - n:]
-            cur.append((slot, take))
-            n += len(take)
-    if cur:
-        launches.append(cur)
-    for members in launches:
-        B = len(members)
-        off, flat = [0], []
-        for _, rs in members:
-            flat += [v for r in rs for v in r]
-            off.append(off[-1] + len(rs))
-        _lib.check(lib.m3r_mem_compact_rows(bufs, depth, B, arena.width, arena.cap,
-                                            (C.c_int64 * B)(*[s * arena.cap for s, _ in members]),
-                                            (C.c_int32 * (B + 1))(*off), (C.c_int32 * len(flat))(*flat), stream),
-                   "mem_compact_rows")
-
-
-def _commit(arena, run, new, edits, keep, stream):
-    """The staged rows that stay, per group of adjacent scenes of the call writing the same staged rows."""
-    groups = []
-    for i, s in enumerate(run):
-        w = edits[s].write
-        if w is None:
-            continue
-        if groups and groups[-1][-1][0] == i - 1 and (groups[-1][-1][2][0], groups[-1][-1][2][2]) == (w[0], w[2]):
-            groups[-1].append((i, s, w))
-        else:
-            groups.append([(i, s, w)])
-    for g in groups:
-        i0, i1 = g[0][0], g[-1][0] + 1
-        row0, rows = g[0][2][0], g[0][2][2]
-        _commit_rows(arena, [t[i0:i1] for t in new], [s for _, s, _ in g], row0, rows, [w[1] for _, _, w in g], keep,
-                     stream)
 
 
 def _postprocess(parts, act, out):
@@ -341,8 +283,6 @@ def _run(encoder, decoder, plans, imgs, device, act, max_bs, keyframe_interval, 
         arena.ensure(max(p.max_rows(is_keyframe) for p in plans))
     else:
         searchers = [get_searcher(SEARCHER) for _ in plans]
-    keep = torch.ones(1, dtype=torch.int32, device=dev)
-    stream = cm.stream_ptr(dev)
     results = [{} for _ in plans]
     pending = []                # per step of the last pass, the pointmaps still to postprocess (_postprocess's parts)
     passes = plans[0].passes
@@ -360,8 +300,7 @@ def _run(encoder, decoder, plans, imgs, device, act, max_bs, keyframe_interval, 
                 if it == 0 and k == 0:
                     new, pms = decoder.update_tokens(xs, ps, ts, current_mem=None)
                 else:
-                    mem = ([b[run[0]:run[-1] + 1] for b in arena.bufs], None, 0, 0, 0)
-                    new, pms = decoder.update_tokens(xs, ps, ts, current_mem=mem,
+                    new, pms = decoder.update_tokens(xs, ps, ts, current_mem=arena.memory(run),
                                                      mem_lengths=[arena.lengths[s] for s in run])
                 staged.append((run, new))
                 for g, pm in enumerate(pms):
@@ -392,15 +331,7 @@ def _run(encoder, decoder, plans, imgs, device, act, max_bs, keyframe_interval, 
                 edits = {s: plans[s].step(it, k, is_keyframe) for s in stepping}
             else:
                 edits = {s: plans[s].step(it, k, lambda vid, s=s: decided[(s, vid)]) for s in stepping}
-            runs_of = {s: e.runs for s, e in edits.items() if e.runs}
-            if runs_of:
-                _phase("compact")
-                _compact_rows(arena, runs_of, stream)
-            _phase("memory")
-            for run, new in staged:
-                _commit(arena, run, new, edits, keep, stream)
-            for s, e in edits.items():
-                arena.lengths[s] = e.length
+            apply_edits(arena, staged, edits, _phase)
     _phase("postprocess")
     for parts in pending:
         _postprocess(parts, act, results)

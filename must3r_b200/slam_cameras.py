@@ -24,14 +24,15 @@ import torch
 
 from . import slam as single
 from .engine.frames import AutoMultiLoader, ReadAhead, image_size, schedule
-from .engine.slam_cameras import MAX_CAMERAS, MultiCameraSLAM, steps_of
+from .engine.lockstep import MAX_COMMIT
+from .engine.slam_cameras import MultiCameraSLAM, steps_of
 
 
 def parse_args(argv=None):
     """`python -m must3r_b200.slam`'s parser and checks, then the checks of a shared-map run."""
     args = single.parse_args(argv)
-    if len(args.input) > MAX_CAMERAS:
-        single.get_args_parser().error(f"--input: at most {MAX_CAMERAS} folders")
+    if len(args.input) > MAX_COMMIT:
+        single.get_args_parser().error(f"--input: at most {MAX_COMMIT} folders")
     if args.rerender and len(args.input) > 1:
         single.get_args_parser().error("--rerender with several --input folders is not supported (the reference's "
                                        "rerender_all_frames takes one agent only)")

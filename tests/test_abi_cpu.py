@@ -18,7 +18,7 @@ def declared_functions():
     return sorted(set(re.findall(r"\b(m3r_[a-z0-9_]+)\s*\(", src)))
 
 
-def test_library_builds_and_exports_every_declared_symbol():
+def test_library_builds_at_abi_5_and_exports_every_declared_symbol():
     import __graft_entry__ as g
     g.build()
     from must3r_b200 import _lib
@@ -29,7 +29,7 @@ def test_library_builds_and_exports_every_declared_symbol():
     for n in names:
         assert hasattr(lib, n), f"{n} declared in the header but not exported"
         assert n in _lib.SIGNATURES, f"{n} has no ctypes signature"
-    assert lib.m3r_abi_version() == 4
+    assert lib.m3r_abi_version() == 5
 
 
 def test_ctypes_structs_match_the_c_layout(tmp_path):

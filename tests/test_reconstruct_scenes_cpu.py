@@ -4,8 +4,8 @@ import pytest
 
 from must3r_b200 import reconstruct, reconstruct_scenes as cli
 from must3r_b200.engine import demo
-from must3r_b200.engine.scenes import (ScenePlan, arena_rows, lockstep_calls, plan_memory_calls, plan_render_calls,
-                                       signature)
+from must3r_b200.engine.lockstep import StepEdit, lockstep_calls, signature
+from must3r_b200.engine.scenes import ScenePlan, arena_rows, plan_memory_calls, plan_render_calls
 
 L, P = (288, 384), (384, 288)          # landscape, portrait (H, W)
 NL, NP = 18 * 24, 24 * 18              # tokens per view
@@ -87,6 +87,20 @@ def test_refresh_rows_skip_the_reference_view():
     # re-run of the init step: staged rows [NL, 2 NL) over memory rows [NL, 2 NL); later steps whole
     assert p.refresh_row0(0) == NL and p.step_start[0] + p.refresh_row0(0) == NL
     assert p.refresh_row0(1) == 0 and p.step_start[1] == 2 * NL
+
+
+def test_step_edits_write_behind_and_skip_the_reference_view():
+    """ScenePlan.step: pass 0 appends each step's rows behind the memory; a refinement pass rewrites them in place, but
+    never the reference view's rows [0, NL)."""
+    p = ScenePlan(files(5), [L] * 5, 3, max_bs=None)
+    assert p.step(0, 0) == StepEdit([], (0, 0, 2 * NL), 2 * NL)
+    assert p.step(0, 1) == StepEdit([], (0, 2 * NL, NL), 3 * NL)
+    assert p.step(1, 0) == StepEdit([], (NL, NL, NL), 3 * NL)
+    assert p.step(1, 1) == StepEdit([], (0, 2 * NL, NL), 3 * NL)
+    assert all(p.step(it, k).write[1] >= NL for it in (1, 2) for k in range(2))
+    init_mixed = ScenePlan(files(2), [P, L], 2, max_bs=None)        # the landscape reference view stays
+    assert init_mixed.step(0, 0) == StepEdit([], (0, 0, NL + NP), NL + NP)
+    assert init_mixed.step(1, 0) == StepEdit([], (NL, NL, NP), NL + NP)
 
 
 def test_cli_parsing_and_rejections(capsys):

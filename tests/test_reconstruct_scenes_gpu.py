@@ -16,7 +16,7 @@ import torch
 
 from must3r_b200 import _lib
 from must3r_b200 import synthetic as syn
-from must3r_b200.engine import demo, scenes
+from must3r_b200.engine import demo, lockstep, scenes
 from must3r_b200.model import common as cm
 from must3r_b200.model import load_model
 
@@ -64,7 +64,7 @@ def feats(files, model):
 
 
 def shape(hw, B, n):
-    return scenes._host_shape(hw, B, n)
+    return lockstep._host_shape(hw, B, n)
 
 
 def memories(dec, feats, n_views):
@@ -101,7 +101,7 @@ def precision():
 
 # ------------------------------------------------------------------------------------------------ kernels
 @pytest.mark.parametrize("dtype", PRECISIONS, ids=["fp16", "bf16", "fp8"])
-def test_render_tokens_equal_lengths_is_forward_render(model, feats, dtype, precision):
+def test_ragged_render_of_equal_lengths_is_forward_render(model, feats, dtype, precision):
     precision(dtype)
     dec = model[1]
     arena, lens = memories(dec, feats, [2, 2, 2])
@@ -115,7 +115,7 @@ def test_render_tokens_equal_lengths_is_forward_render(model, feats, dtype, prec
 
 
 @pytest.mark.parametrize("dtype", PRECISIONS, ids=["fp16", "bf16", "fp8"])
-def test_render_tokens_unequal_lengths_match_each_scene_alone(model, feats, dtype, precision):
+def test_ragged_render_of_unequal_lengths_matches_each_scene_alone(model, feats, dtype, precision):
     """Scenes of 1, 4, 2 and 3 views, rows past each length NaN (then +inf, then -inf: the same bits); each scene's render
     is its own render against its memory truncated to its length, and the memory is bitwise unchanged."""
     precision(dtype)
@@ -141,7 +141,7 @@ def test_render_tokens_unequal_lengths_match_each_scene_alone(model, feats, dtyp
         assert torch.equal(again, got), fill
 
 
-def test_render_tokens_argument_checks(model, feats):
+def test_ragged_render_argument_checks(model, feats):
     dec = model[1]
     arena, lens = memories(dec, feats, [1, 2])
     x, pos, ts = queries(feats, 2, 1)

@@ -9,7 +9,7 @@ import torch
 
 from helpers import tiny_oracle
 from must3r_b200 import engine, reconstruct, reconstruct_videos as cli, synthetic as syn
-from must3r_b200.engine import videos
+from must3r_b200.engine import lockstep, videos
 from must3r_b200.engine.videos import VideoPlan, plan_step_calls
 from oracle import must3r_oracle as orc
 
@@ -107,7 +107,7 @@ def test_edits_of_a_steady_window():
     q = VideoPlan([SHAPES[0]] * 4, 0)
     q.step(0, 0)
     e = q.step(0, 1, lambda v: False)
-    assert e == videos.StepEdit([], None, 2 * N)
+    assert e == lockstep.StepEdit([], None, 2 * N)
 
 
 def test_lockstep_calls_of_videos():
@@ -126,7 +126,7 @@ def test_lockstep_calls_of_videos():
     assert plan_step_calls([VideoPlan([L] * 4), VideoPlan([L] * 2)], 0) == [(((L, 2),), [0, 1])]
 
 
-def test_compaction_runs_split_over_launches(monkeypatch):
+def test_compact_splits_runs_over_launches(monkeypatch):
     """More runs than one launch takes: every scene's runs go out in order, a scene cut at a launch boundary goes on in
     the next launch, and each launch's base rows are its slots' (ascending)."""
     calls = []
@@ -138,13 +138,14 @@ def test_compaction_runs_split_over_launches(monkeypatch):
             calls.append((list(base[:B]), [[tuple(flat[3 * k:3 * k + 3]) for k in range(off[b], off[b + 1])]
                                            for b in range(B)]))
             return 0
-    monkeypatch.setattr(videos._lib, "lib", lambda: Lib())
+    monkeypatch.setattr(lockstep._lib, "lib", lambda: Lib())
+    monkeypatch.setattr(lockstep.cm, "stream_ptr", lambda device: C.c_void_p(0))
 
     class Arena:
-        depth, width, cap = 2, 64, 10000
+        depth, width, cap, device = 2, 64, 10000, torch.device("cpu")
         bufs = [torch.zeros(1), torch.zeros(1)]
     runs_of = {s: [(100 * k + 50, 100 * k, 10) for k in range(n)] for s, n in ((0, 5), (3, 200), (7, 60))}
-    videos._compact_rows(Arena(), runs_of, C.c_void_p(0))
+    lockstep.compact(Arena(), runs_of)
     assert [len(sum(r, [])) for _, r in calls] == [128, 128, 9]
     got = {}
     for base, per_scene in calls:

@@ -16,8 +16,8 @@ import torch
 
 from must3r_b200 import _lib
 from must3r_b200 import synthetic as syn
-from must3r_b200.engine import demo, videos
-from must3r_b200.engine.slam_sessions import SessionArena
+from must3r_b200.engine import demo, lockstep, videos
+from must3r_b200.engine.lockstep import SessionArena
 from must3r_b200.model import common as cm
 from must3r_b200.model import load_model
 
@@ -141,8 +141,8 @@ def test_compaction_of_64_slots(dtype):
         check_compaction(dtype, 64, cap, width, runs, list(range(64)), seed=width)
 
 
-def test_compaction_runs_past_one_launch():
-    """videos._compact_rows cuts 300 runs of one scene and 5 of another over launches; the result is the sequential one."""
+def test_compact_runs_past_one_launch():
+    """lockstep.compact cuts 300 runs of one scene and 5 of another over launches; the result is the sequential one."""
     arena = SessionArena(3, 2, 64, torch.float16, "cuda")
     arena.ensure(4000)
     for b in arena.bufs:
@@ -153,7 +153,7 @@ def test_compaction_runs_past_one_launch():
         for s, rs in runs_of.items():
             for src, dst, n in rs:
                 w[s, dst:dst + n] = w[s, src:src + n].clone()
-    videos._compact_rows(arena, runs_of, cm.stream_ptr(torch.device("cuda")))
+    lockstep.compact(arena, runs_of)
     torch.cuda.synchronize()
     for a, w in zip(arena.bufs, want):
         assert torch.equal(a.view(torch.int16), w.view(torch.int16))

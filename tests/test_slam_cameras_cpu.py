@@ -12,7 +12,7 @@ from must3r_b200 import slam as single
 from must3r_b200 import slam_cameras as cli
 from must3r_b200.engine import frames
 from must3r_b200.engine.slam_cameras import commit_rows, steps_of
-from must3r_b200.engine.slam_sessions import plan_batch
+from must3r_b200.engine.lockstep import plan_batch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
@@ -115,7 +115,7 @@ def test_batching_plan():
 
 # ------------------------------------------------------------------------------------------------ ordered commit rows
 def _restated(keyframe, row0, N, depth=2, width=8, cap=64, seed=0):
-    """The ordered commit applied to a numpy memory the way sequential m3r_mem_commit calls would: frame after frame,
+    """The ordered commit applied to a numpy memory the way sequential m3r_mem_commit_rows calls would: frame after frame,
     a keyframe's rows at the current end."""
     rng = np.random.default_rng(seed)
     mem = rng.standard_normal((depth, cap, width))

@@ -42,8 +42,8 @@ def _ptrs(ts):
 
 @pytest.mark.parametrize("flags", [[1, 1, 1, 1], [0, 0, 0, 0], [1, 0, 1, 0], [0, 0, 0, 1]],
                          ids=["all", "none", "alternating", "last"])
-def test_ordered_commit_is_sequential_commits(flags):
-    """m3r_mem_commit_ordered with the flags in records (stride 3 ints) = m3r_mem_commit frame after frame with the
+def test_ordered_commit_is_sequential_commit_rows(flags):
+    """m3r_mem_commit_ordered with the flags in records (stride 3 ints) = m3r_mem_commit_rows frame after frame with the
     rows counted on the host; every row past the new length (guard rows) keeps its sentinel."""
     depth, cap, W, F, Nt, row0 = 3, 40, 256, len(flags), 5, 7
     arena = [torch.full((1, cap, W), 7.0, dtype=torch.float16, device="cuda") for _ in range(depth)]
@@ -56,8 +56,8 @@ def test_ordered_commit_is_sequential_commits(flags):
     n = row0
     for k, f in enumerate(flags):
         one = [t[k:k + 1] for t in staged]
-        rc = lib.m3r_mem_commit(_ptrs(want), _ptrs(one), depth, 1, Nt, W, (C.c_int64 * 1)(n),
-                                C.c_void_p(keep.data_ptr() + 12 * k), 0, stream)
+        rc = lib.m3r_mem_commit_rows(_ptrs(want), _ptrs(one), depth, 1, 0, Nt, Nt, W, (C.c_int64 * 1)(n),
+                                     C.c_void_p(keep.data_ptr() + 12 * k), 0, stream)
         assert rc == 0
         n += Nt if f else 0
     torch.cuda.synchronize()

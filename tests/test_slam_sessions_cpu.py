@@ -1,11 +1,17 @@
 """Host bookkeeping of the multi-session SLAM (must3r_b200/engine/slam_sessions.py): the arena's slots and growth, the
-batching rule, and the command line's arguments.  No GPU."""
+batching rule, the split of a keyframe commit over launches, and the command line's arguments.  No GPU."""
+import ctypes as C
+from types import SimpleNamespace
+
 import pytest
 import torch
 
+from must3r_b200 import ops
 from must3r_b200 import slam as single
 from must3r_b200 import slam_sessions as cli
-from must3r_b200.engine.slam_sessions import SessionArena, plan_batch, slot_runs
+from must3r_b200.engine import lockstep
+from must3r_b200.engine.lockstep import SessionArena, plan_batch, slot_runs
+from must3r_b200.engine.slam_sessions import SLAMSessions
 
 
 def test_arena_slots_and_growth():
@@ -41,6 +47,35 @@ def test_batching_rule():
     assert plan_batch({}) == ([], [])
     assert slot_runs([0, 1, 2]) == [[0, 1, 2]]
     assert slot_runs([0, 2, 3, 5]) == [[0], [2, 3], [5]]
+
+
+def test_keyframe_commit_of_70_sessions_splits_over_launches(monkeypatch):
+    """One run of 70 consecutive slots commits in launches of at most 64 sessions: each launch gets its sessions'
+    staged blocks, their rows behind each memory, and the keyframe flag of its first session's record."""
+    calls = []
+
+    class Lib:
+        def m3r_mem_commit_rows(self, arena, staged, depth, B, row0, rows, stride, width, dst, keep, keep_stride, stream):
+            assert B <= 64 and (depth, row0, rows, stride, width) == (2, 0, 3, 3, 8)
+            calls.append((B, staged[0], list(dst[:B]), keep.value, keep_stride))
+            return 0
+    monkeypatch.setattr(lockstep._lib, "lib", lambda: Lib())
+    monkeypatch.setattr(lockstep.cm, "stream_ptr", lambda device: C.c_void_p(0))
+    ss = SLAMSessions.__new__(SLAMSessions)              # only the arena and the slots: no model
+    ss.arena = SessionArena(72, depth=2, width=8, dtype=torch.float16, device="cpu")
+    ss.arena.ensure(20)
+    ss.sessions = [SimpleNamespace(slot=s) for s in range(72)]
+    members = list(range(1, 71))
+    ss.arena.lengths = [s % 5 for s in range(72)]
+    staged = [torch.zeros(70, 3, 8, dtype=torch.float16) for _ in range(2)]
+    recs = torch.zeros((70, ops.SLAM_RECORD.itemsize), dtype=torch.uint8)
+    ss._commit([(members, staged)], recs, {sid: i for i, sid in enumerate(members)})
+    flag = ops.SLAM_RECORD.fields["keyframe"][1]
+    assert [c[0] for c in calls] == [64, 6]
+    for (B, src, dst, keep, stride), lo in zip(calls, (0, 64)):
+        assert src == staged[0][lo].data_ptr()
+        assert dst == [s * 20 + s % 5 for s in members[lo:lo + B]]
+        assert keep == recs.data_ptr() + lo * ops.SLAM_RECORD.itemsize + flag and stride == ops.SLAM_RECORD.itemsize // 4
 
 
 def test_cli_arguments(tmp_path):

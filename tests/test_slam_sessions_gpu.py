@@ -116,11 +116,13 @@ def commit(arena, staged, dst_rows, keep, stride, keep_byte_offset=0):
     a = (C.c_void_p * len(arena))(*[t.data_ptr() for t in arena])
     s = (C.c_void_p * len(staged))(*[t.data_ptr() for t in staged])
     rows = (C.c_int64 * len(dst_rows))(*dst_rows)
-    return lib.m3r_mem_commit(a, s, len(arena), staged[0].shape[0], staged[0].shape[1], staged[0].shape[2], rows,
-                              C.c_void_p(keep.data_ptr() + keep_byte_offset), stride, cm.stream_ptr(torch.device("cuda")))
+    Nt = staged[0].shape[1]
+    return lib.m3r_mem_commit_rows(a, s, len(arena), staged[0].shape[0], 0, Nt, Nt, staged[0].shape[2], rows,
+                                   C.c_void_p(keep.data_ptr() + keep_byte_offset), stride,
+                                   cm.stream_ptr(torch.device("cuda")))
 
 
-def test_mem_commit_writes_exactly_the_selected_rows():
+def test_mem_commit_rows_appends_exactly_the_flagged_rows():
     S, cap, W, B, Nt, depth = 4, 50, 256, 3, 7, 3
     sentinel = 7.0
     arena = [torch.full((S, cap, W), sentinel, dtype=torch.float16, device="cuda") for _ in range(depth)]

@@ -45,7 +45,7 @@ def run_batched(chkpt, seqs, warmup, res):
     mc = scm.MultiCameraSLAM(chkpt, K, device="cuda:0", res=res)
     enc = mc.model[0]
     marks = []
-    fwd, dec, com = enc.forward, scm.MultiCameraSLAM._decode_shared, scm.MultiCameraSLAM._commit_ordered
+    fwd, dec, com = enc.forward, scm.MultiCameraSLAM._decode_shared, scm.commit_ordered
 
     def timed_encoder(*a, **k):
         marks.append([ev()])
@@ -58,13 +58,12 @@ def run_batched(chkpt, seqs, warmup, res):
         marks[-1].append(ev())
         return out
 
-    def timed_commit(self, *a, **k):
+    def timed_commit(*a, **k):
         marks[-1].append(ev())
-        com(self, *a, **k)
+        com(*a, **k)
         marks[-1].append(ev())
 
-    enc.forward, scm.MultiCameraSLAM._decode_shared, scm.MultiCameraSLAM._commit_ordered = \
-        timed_encoder, timed_decode, timed_commit
+    enc.forward, scm.MultiCameraSLAM._decode_shared, scm.commit_ordered = timed_encoder, timed_decode, timed_commit
     try:
         for k in range(warmup):
             mc.step({c: (seq[k], k * K + c) for c, seq in enumerate(seqs)})
@@ -77,7 +76,7 @@ def run_batched(chkpt, seqs, warmup, res):
         wall = time.perf_counter() - t0
     finally:
         del enc.forward
-        scm.MultiCameraSLAM._decode_shared, scm.MultiCameraSLAM._commit_ordered = dec, com
+        scm.MultiCameraSLAM._decode_shared, scm.commit_ordered = dec, com
     full = [m for m in marks if len(m) == 5]
     split = {name: round(float(np.median([m[i].elapsed_time(m[i + 1]) for m in full])), 3) if full else None
              for i, name in enumerate(("encoder_ms", "decoder_ms", "tail_ms", "commit_ms"))}
